@@ -25,6 +25,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -37,14 +38,24 @@ MODULI = [0x7fffffd8001, 0x7fffffc8001, 0xfffffffc001, 0xffffff6c001, 0xfffffebc
 PLAIN = 1032193
 BATCH = 1024
 NTT_POLYS = 4096  # BASELINE config 2
+DUMP_ITEMS = 32  # --dump-outputs: ciphertexts sampled from the batch (32 x 2 x 4 x 8192 float64 words = 16 MiB)
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
+
+
+def dump_outputs(directory, out):
+    """Writes a fixed, seeded sample of the last timed step's products as float64 .npy files (every residue is below 2^53,
+    so the conversion is exact), so that two builds can be compared output for output."""
+    import numpy as np
+    import torch
+    os.makedirs(directory, exist_ok=True)
+    B = out.shape[0]
+    idx = np.sort(np.random.default_rng(0).choice(B, size=min(DUMP_ITEMS, B), replace=False))
+    words = out[torch.from_numpy(idx).to(out.device)].cpu().numpy().view(np.uint64)
+    np.save(os.path.join(directory, "mul_relin_out.npy"), words.astype(np.float64))
+    np.save(os.path.join(directory, "mul_relin_out_items.npy"), idx.astype(np.float64))
 
 
 def cpu_quota():
@@ -197,7 +208,7 @@ def run_reference(args):
                                    "uniform-random ciphertext words",
                          # threads used vs what the lease really grants (a CPU-quota'd 1-GPU lease gives ~16 cores' worth)
                          "box": cpu_quota(),
-                         "build": "unmodified reference sources, -O3, Intel HEXL off (not buildable offline)"},
+                         "build": "unmodified reference sources, -O3, Intel HEXL off"},
         "e2e": {"value": rate, "unit": "ops/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
     print(json.dumps(line))
@@ -285,6 +296,8 @@ class PluginLegs:
         src = os.path.join(ROOT, "tools", "plugin_probe.cpp")
         try:
             if not os.path.exists(so) or os.path.getmtime(so) < os.path.getmtime(src):
+                # the tree may be read-only: a missing or stale harness is compiled outside it
+                so = os.path.join(tempfile.mkdtemp(prefix="plugin_probe_"), "libplugin_probe.so")
                 subprocess.run(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-pthread", "-o", so, src], check=True)
             C = self.C
             lib = C.CDLL(so)
@@ -347,7 +360,8 @@ def main():
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--batch", type=int, default=BATCH)
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
-    ap.add_argument("--quick", action="store_true", help="device-resident loop + rooflines only (for runs under ncu)")
+    ap.add_argument("--quick", action="store_true", help="device-resident loop + rooflines only")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a fixed sample of the last timed step's outputs as .npy files")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -360,7 +374,7 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device: the B200 backend has no CPU fallback")
+        raise SystemExit("bench.py needs a CUDA device: the CUDA backend has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     numa_node = None if os.environ.get("B200_BENCH_NO_NUMA") else bind_to_gpu_numa(local)
@@ -424,6 +438,8 @@ def main():
         dist.all_reduce(tms, op=dist.ReduceOp.MAX)
         ms = float(tms.item())
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     value = world * B * args.steps / (ms / 1000.0)
 
     ct_bytes = 2 * k * n * 8
@@ -483,8 +499,7 @@ def main():
         link["bidir_d2h_gbs"] = 2 * out.numel() * 8 / (ev[2].elapsed_time(ev[3]) / 1000.0) / 1e9
         ah.copy_(a)  # (a was only overwritten with its own contents; keep the pinned copy authoritative)
         # ceiling of the e2e legs (2 ct in, 1 ct out per op): each direction at its own rate with every rank copying, and both
-        # together within what the host sustains when every rank moves data BOTH ways at once (on the 8-GPU node that sum is
-        # ~49 GB/s per GPU against 54 + 40 one way: the host side, not the links, bounds the scaling of `e2e`)
+        # together within what the host sustains when every rank moves data BOTH ways at once
         link["bound_ops_per_s"] = min(link["h2d_gbs"] * 1e9 / (2 * ct_bytes), link["d2h_gbs"] * 1e9 / ct_bytes,
                                       (link["bidir_h2d_gbs"] + link["bidir_d2h_gbs"]) * 1e9 / (3 * ct_bytes))
 
@@ -680,8 +695,7 @@ def main():
                        "single_thread_ops_per_s": rate1,
                        # a CPU-quota'd lease shows up here: threads >> the cores' worth of time the box grants
                        "box": quota, "parallel_speedup_over_one_thread": rate / rate1 if rate1 else None,
-                       "build": "unmodified reference sources, -O3, Intel HEXL off (not buildable offline), one MemoryPool per thread",
-                       "full_node_reference": "the same arm on an 8-GPU lease (96-core cgroup quota, 128 threads): 3654 ops/s (profiles/r2_bench_reference_arm_fullnode.json)"}
+                       "build": "unmodified reference sources, -O3, Intel HEXL off, one MemoryPool per thread"}
             except Exception as ex:  # reference .so missing on this box
                 cpu = {"value": None, "unit": "ops/s", "cores": os.cpu_count(), "kind": "reference",
                        "sample": f"unavailable: {ex}"}
@@ -697,7 +711,7 @@ def main():
             "config": {"workload": "Evaluator::multiply + relinearize, n=8192, BFVDefault 218-bit chain (k=4 + special), "
                                    f"batch={B} ct pairs per GPU", "batch_per_gpu": B,
                        "parallelism": f"batch sharded over {world} GPU(s), no data-path collective",
-                       "l2": "inputs (1 GiB per GPU) exceed the 126 MB L2; no explicit flush"},
+                       "l2": "inputs (1 GiB per GPU) exceed the 50 MB L2; no explicit flush"},
             "clocks": clocks, "gpu_launches": int(launches),
             "e2e": {"value": e2e_value, "unit": "ops/s",
                     "path": "pinned host words -> B200_Ciphertext_SetWordsBatch -> B200_Evaluator_MultiplyRelinBatch -> "

@@ -1,4 +1,4 @@
-"""sunscreen_b200 — a B200-native BFV ciphertext-arithmetic backend behind Sunscreen's `seal_fhe` FFI.
+"""sunscreen_b200 — an H100-native BFV ciphertext-arithmetic backend behind Sunscreen's `seal_fhe` FFI.
 
 The product is the CUDA shared library `libb200bfv.so` (built in-tree from `csrc/`); the Python modules are plumbing:
     lib       ctypes binding of the layer-1 "slab" C ABI        (include/b200_bfv.h)

@@ -1,4 +1,4 @@
-// b200_bfv.cu — CUDA kernels (sm_100a), device context and the layer-1 C ABI (include/b200_bfv.h).
+// b200_bfv.cu — CUDA kernels (sm_90a), device context and the layer-1 C ABI (include/b200_bfv.h).
 //
 // One process drives one GPU.  All work is enqueued on the caller's stream; temporaries come from the
 // context-private stream-ordered pool (cudaMallocFromPoolAsync), so back-to-back calls never synchronise with the host.
@@ -1324,7 +1324,7 @@ static int launch_ntt(b200_ctx *ctx, const JobDesc &jd, const u64 *src, long lon
         static const int nt_env = std::getenv("B200_NTT_NT") ? atoi(std::getenv("B200_NTT_NT")) : 0;
         int var_env = g_ntt_var.load(std::memory_order_relaxed);
         if (var_env < 0)
-        { // automatic: what measured fastest per size and direction (profiles/r2_ntt_variants.txt).  2048 = warp(-group)-private
+        { // automatic: what measured fastest per size and direction (tools/ntt_ablate.py).  2048 = warp(-group)-private
           // sub-transforms, +1 = first 512 twiddles in shared memory, +16 = streaming (persistent) kernel
             if (ctx->logn == 14)
                 var_env = FWD ? 2049 : 2064;
@@ -1826,7 +1826,7 @@ int b200_ctx_create(uint64_t n, const uint64_t *coeff_modulus, uint64_t count, u
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0)
-        return fail(B200_E_CUDA, "no CUDA device available: the B200 backend has no CPU fallback");
+        return fail(B200_E_CUDA, "no CUDA device available: the CUDA backend has no CPU fallback");
     if (device < 0 || device >= ndev)
         return fail(B200_E_INVALID, "device index out of range");
     CU_TRY(cudaSetDevice(device));
@@ -3216,9 +3216,8 @@ static void cpu_unpack48(HostPool *pool, const uint8_t *src, u64 *dst, size_t wo
 
 static bool level_packs(const b200_ctx *ctx, int level)
 {
-    // Opt-in (B200_HOST_PACK=1).  Measured on the pool's hosts (profiles/r1_e2e_packing.txt): narrowing on the CPU costs
-    // more host memory traffic (~5 GiB per 1024 ops instead of 1.5) than PCIe saves — 31 k ops/s with 16 packing
-    // threads against 46.5 k ops/s for plain pinned DMA — so the default is the plain pipeline.
+    // Opt-in (B200_HOST_PACK=1).  Narrowing on the CPU costs more host memory traffic (~5 GiB per 1024 ops instead of 1.5)
+    // than PCIe saves, so the default is the plain pipeline.
     const char *e = getenv("B200_HOST_PACK");
     if (!e || atoi(e) == 0 || (ctx->n & 3))
         return false;

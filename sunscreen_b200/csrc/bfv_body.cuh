@@ -451,7 +451,7 @@ B200_HD u64 decrypt_coeff(const LevelDev &L, const u64 *__restrict__ src, long l
 
 
 // =========================================================================================================
-// FP64-pipe variants (B200: DFMA issues 2.5x faster than IMAD.WIDE; see ntt_fp_body.cuh for the exactness
+// FP64-pipe variants (the wide integer multiply is the slower pipe; see ntt_fp_body.cuh for the rationale and the exactness
 // argument).  Same mathematics, same canonical outputs; used when LevelDev::fp is set.
 // =========================================================================================================
 B200_HD double fp_canon(double r, double p) // (-p, p) -> [0, p)
@@ -470,8 +470,8 @@ B200_HD double ldd(const double *p) { return B200_LDG(p); }
 
 // BEHZ constants of the FP64 path, passed BY VALUE as a kernel parameter: they live in the constant bank, so each
 // use is a constant operand of the DFMA/DMUL itself (or one uniform load) instead of a global load through L1 —
-// with ~70 (lift) / ~140 (scale) constants per coefficient the pointer-based version kept L1TEX at 62 % busy and the
-// FP64 pipe at 47-53 % (profiles/r1_ncu_elementwise.txt).  Entries are {w, w/p_target} pairs, primes {p, 1/p}.
+// with ~70 (lift) / ~140 (scale) constants per coefficient the pointer-based version kept L1TEX busy and starved the
+// FP64 pipe.  Entries are {w, w/p_target} pairs, primes {p, 1/p}.
 template <int K>
 struct LiftFpC
 {

@@ -1,4 +1,4 @@
-// ksmac_tma.cu — key-switch inner product with TMA-tiled key streaming (sm_100a).
+// ksmac_tma.cu — key-switch inner product with TMA-tiled key streaming (sm_90a).
 //
 // What it computes (reference: the MAC loop of switch_key_inplace, S/evaluator.cpp:2517-2541, key layout S/kswitchkeys.h:340):
 //     acc_c[I][coeff] = sum_J  NTT_{p_I}(digit_J)[coeff] * key[J][c][I][coeff]   (mod p_I),   c in {0,1}, I in [0,k] (I = k: special prime)

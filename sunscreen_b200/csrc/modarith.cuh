@@ -1,4 +1,4 @@
-// modarith.cuh — 64-bit modular arithmetic primitives for sm_100a (host/device).
+// modarith.cuh — 64-bit modular arithmetic primitives for sm_90a (host/device).
 //
 // Everything here is exact unsigned integer arithmetic; "lazy" variants document their output range.
 // Semantics follow the reference's scalar helpers (results, not code):

@@ -1,7 +1,7 @@
-// ntt_fp_body.cuh — the FP64-pipe negacyclic NTT / INTT for primes below 2^47 (B200-specific fast path).
+// ntt_fp_body.cuh — the FP64-pipe negacyclic NTT / INTT for primes below 2^47 (fast path for GPUs with a full-rate FP64 pipe).
 //
-// Why: on B200 (sm_100a) the 64-bit integer butterfly is bound by IMAD.WIDE.U32, which issues at only ~25
-// lanes/clk/SM (measured, tools/ubench.cu), while DFMA/DMUL/DADD issue at 64 lanes/clk/SM.  A modular
+// Why: the 64-bit integer butterfly is bound by the wide integer multiply (IMAD.WIDE.U32 / IMAD.HI chains; tools/ubench.cu
+// measures the pipe rates), while H100 issues DFMA/DMUL/DADD at 64 lanes/clk/SM (its full-rate FP64 pipe).  A modular
 // multiplication by a precomputed twiddle can be done EXACTLY in 6 double-precision operations:
 //     h = y*w (rounded)            l = fma(y, w, -h)        (h + l == y*w exactly)
 //     q = rint(h * (1/p))          (DMUL + FRND.F64; the rounding runs on the XU pipe, not the FP64 pipe)
@@ -726,7 +726,7 @@ struct NttFpStaticPass
                     else if constexpr (L <= 3 && NGROUPS % NT == 0 && ITERS > 1 && B200_NTT_TW_PREFETCH && TWSRC == 0)
                     {
                         // the twiddles of group it+1 are requested before group `it` is transformed: their L1/L2 latency
-                        // (the largest stall reason of the kernel, profiles/r1_ncu_ntt_v6.txt) overlaps the butterflies
+                        // (the kernel's largest stall reason when profiled) overlaps the butterflies
                         constexpr int R = 1 << L;
                         const double *__restrict__ twt = FWD ? P.fwd : P.inv;
                         double twc[R - 1], twn[R - 1];

@@ -146,7 +146,7 @@ struct Context_
     static const int GRAPHS_PER_LANE = 48;
     bool use_graphs = true; // B200_NO_GRAPHS=1: enqueue the kernels one by one
     // B200_BLOCKING_WAITS=1: the batch seams sleep on a blocking-sync event instead of spinning in cudaStreamSynchronize.  Off by
-    // default: measured on the B200 boxes the sleeping wait halves the throughput of the chunked host-buffer pipeline (wake-up latency
+    // default: the sleeping wait was measured to halve the throughput of the chunked host-buffer pipeline (wake-up latency
     // of the order of a chunk's run time); it exists for hosts where caller threads outnumber the cores the process is granted.
     bool blocking_waits = false;
     static const int NLANE = 8;

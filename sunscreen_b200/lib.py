@@ -1,9 +1,9 @@
 """ctypes binding of the layer-1 C ABI (include/b200_bfv.h) — plumbing, not the product.
 
-The product is sunscreen_b200/libb200bfv.so (CUDA, sm_100a).  This module only loads it, declares the
+The product is sunscreen_b200/libb200bfv.so (CUDA, sm_90a).  This module only loads it, declares the
 signatures and turns error codes into exceptions; buffers are raw device pointers (ints), typically
 `torch.Tensor.data_ptr()` of a CUDA tensor.  There is no CPU fallback: if the shared library is missing or
-was not built by nvcc for sm_100a, loading fails loudly.
+was not built by nvcc for sm_90a, loading fails loudly.
 """
 import ctypes as C
 import os
@@ -104,7 +104,7 @@ class B200Lib:
         if not os.path.exists(path):
             raise ImportError(
                 f"{path} not found: build it with __graft_entry__.build() / make -C sunscreen_b200/csrc "
-                "(the B200 backend has no CPU fallback)")
+                "(the CUDA backend has no CPU fallback)")
         if not _allow_emu and "emu" in os.path.basename(path):
             raise ImportError("refusing to load a tests/emu build as the product library")
         self.path = path

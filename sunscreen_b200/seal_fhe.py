@@ -1,4 +1,4 @@
-"""Python mirror of the `seal_fhe` Rust crate's public API, bound to the SEAL-named C ABI of the B200 backend.
+"""Python mirror of the `seal_fhe` Rust crate's public API, bound to the SEAL-named C ABI of the CUDA backend.
 
 The image has no Rust toolchain, so this module plays the role of `seal_fhe/src/*.rs`: the same type names, method names,
 argument meaning and error behaviour, implemented with the same FFI calls the Rust wrappers make

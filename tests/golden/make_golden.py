@@ -1,11 +1,12 @@
 #!/usr/bin/env python
 """Regenerates tests/golden/appendix_b.json from the UNMODIFIED reference (oracle/_ref/libsealc_ref.so).
 
-Run in the build container (where /root/reference exists and `make -C oracle ref` has been run):
+Run where the reference sources exist and `make -C oracle ref` has built oracle/_ref/libsealc_ref.so:
     python tests/golden/make_golden.py
 For every parameter set of tests/params.py it fills ciphertexts / plaintext / key-switching keys with the RNG-free
 splitmix64 stream of SURVEY.md App. B, runs each Evaluator entry point of the reference through its C export layer
-and records the FNV-1a-64 of the output words (plus the context constants that pin the host precompute).
+and records the FNV-1a-64 of the output words (plus the context constants that pin the host precompute), and the
+per-prime hashes of the full-size forward NTT of BASELINE config 2 (config2_ntt.json).
 It also writes tests/golden/small_n64.npz: full input/output words at n=64 (sec_level none) for a word-level fixture.
 """
 import json
@@ -64,6 +65,21 @@ def golden_for(n, moduli, t, sec=refseal.SEC_TC128, full=False):
     return out, inp, words
 
 
+def config2_hashes():
+    """BASELINE config 2: FNV-1a-64, per prime, of the reference's forward NTT of 4096 polynomials whose residues are the
+    splitmix64(0xB200) % q_i stream of SURVEY.md App. B (tests/test_gpu_parity.py::test_config2_all_16384_transforms_vs_reference)."""
+    R = refseal.RefLib.get()
+    out = {}
+    for name in ("n8192", "n8192_54"):
+        n, moduli, _ = PARAMS[name]
+        items, state, hashes = 4096, 0xB200, []
+        for i in range(4):
+            w, state = refseal.splitmix64_words(items * n, int(moduli[i]), state)
+            hashes.append("%016x" % refseal.fnv1a64(R.ntt_forward_mt(int(moduli[i]), w.reshape(items, n), os.cpu_count() or 1)))
+        out[name] = hashes
+    return out
+
+
 def main():
     res = {}
     for name, (n, moduli, t) in PARAMS.items():
@@ -71,6 +87,8 @@ def main():
         res[name], _, _ = golden_for(n, moduli, t)
     with open(os.path.join(HERE, "appendix_b.json"), "w") as f:
         json.dump(res, f, indent=1)
+    with open(os.path.join(HERE, "config2_ntt.json"), "w") as f:
+        json.dump(config2_hashes(), f, indent=1)
     # small word-level fixture: n=64, two 30-bit data primes + one special prime, t = 257 (batching-friendly: 257 = 1 mod 128)
     n, t = 64, 257
     P = refseal.RefLib.get()

@@ -1,7 +1,7 @@
 """Word-for-word parity checks of the B200 path against the unmodified reference (shared by CPU-emu and GPU tests)."""
 import numpy as np
 
-from refseal import RefContext, appendix_b_inputs
+from refseal import RefContext, appendix_b_inputs, fnv1a64
 from sunscreen_b200.lib import B200Context
 
 
@@ -160,17 +160,24 @@ def check_relin(P, m3=None, rm=None):
 
 
 def check_galois(P):
+    """Galois automorphisms 3 (rotate rows by 1) and 2n-1 (swap columns).  Without a batching plain modulus the reference
+    refuses rotate_rows / rotate_columns, but Evaluator::apply_galois with the same elements and keys is still defined
+    (S/evaluator.cpp:2217-2307): the comparison is then against that."""
     n = P.n
     a = P.inp["a"]
     ra = P.ref.new_ct(a)
     glk = P.ref.new_ksk({(3 - 1) // 2: P.inp["glk3"], (2 * n - 1 - 1) // 2: P.inp["glkc"]})
     da = P.dev(a)
     o2 = P.out(2, P.k, P.n)
-    assert P.ctx.galois_elt_from_step(1) == 3 and P.ctx.galois_elt_from_step(0) == 2 * n - 1
+    if P.ctx.using_batching:
+        assert P.ctx.galois_elt_from_step(1) == 3 and P.ctx.galois_elt_from_step(0) == 2 * n - 1
+        exp_rows, exp_cols = P.ref.rotate_rows(ra, 1, glk), P.ref.rotate_columns(ra, glk)
+    else:
+        exp_rows, exp_cols = P.ref.apply_galois(ra, 3, glk), P.ref.apply_galois(ra, 2 * n - 1, glk)
     P.ctx.apply_galois(da, 3, P.dev(P.inp["glk3"]), o2, 1)
-    eq(P.host(o2), P.ref.ct_words(P.ref.rotate_rows(ra, 1, glk)), "rotate_rows(1)")
+    eq(P.host(o2), P.ref.ct_words(exp_rows), "galois 3 (rotate_rows(1))")
     P.ctx.apply_galois(da, 2 * n - 1, P.dev(P.inp["glkc"]), o2, 1)
-    eq(P.host(o2), P.ref.ct_words(P.ref.rotate_columns(ra, glk)), "rotate_columns")
+    eq(P.host(o2), P.ref.ct_words(exp_cols), "galois 2n-1 (rotate_columns)")
 
 
 def check_plain(P):
@@ -231,18 +238,30 @@ def check_batch(P, batch=3, seed=7):
             P.ref.free_ct(h)
 
 
+def negacyclic_mul_mod(x, y, t):
+    """x * y in Z_t[X] / (X^n + 1), coefficients of x, y below t < 2^20 (exact in int64 for n <= 32768)."""
+    n = x.size
+    c = np.convolve(x.astype(np.int64), y.astype(np.int64))
+    c = np.concatenate([c, np.zeros(1, dtype=np.int64)])
+    return ((c[:n] % t - c[n:] % t) % t).astype(np.uint64)
+
+
 def check_encrypted_roundtrip(P, seed=3):
-    """Real keys + fresh encryptions from the reference; B200 multiply+relin output decrypts (on the reference
-    AND through b200_decrypt) to the slot-wise product, and equals the reference's ciphertext word for word."""
+    """Real keys + fresh encryptions from the reference; our multiply+relin output decrypts on the reference to the
+    product of the messages (slot-wise for a batching plain modulus, else the negacyclic product of coefficient
+    plaintexts), and equals the reference's ciphertext word for word."""
     rng = np.random.default_rng(seed)
     R = P.ref
     kg = R.keygen()
     sk, pk, rk = R.secret_key(kg), R.public_key(kg), R.relin_keys(kg)
     enc, dec = R.encryptor(pk), R.decryptor(sk)
-    be_ = R.batch_encoder()
     v1 = rng.integers(0, P.t, size=P.n, dtype=np.uint64)
     v2 = rng.integers(0, P.t, size=P.n, dtype=np.uint64)
-    c1, c2 = R.encrypt(enc, R.batch_encode(be_, v1)), R.encrypt(enc, R.batch_encode(be_, v2))
+    if P.ctx.using_batching:
+        be_ = R.batch_encoder()
+        c1, c2 = R.encrypt(enc, R.batch_encode(be_, v1)), R.encrypt(enc, R.batch_encode(be_, v2))
+    else:
+        c1, c2 = R.encrypt(enc, R.new_pt(v1)), R.encrypt(enc, R.new_pt(v2))
     w1, w2 = R.ct_words(c1), R.ct_words(c2)
     key = R.ksk_words(rk)[0]
     exp_ct = R.relinearize(R.multiply(c1, c2), rk)
@@ -252,9 +271,15 @@ def check_encrypted_roundtrip(P, seed=3):
     eq(got, R.ct_words(exp_ct), "multiply_relin on real ciphertexts")
     back = R.new_ct(got.reshape(2, P.k, P.n))
     assert R.noise_budget(dec, back) > 0
-    vals = R.batch_decode(be_, R.decrypt(dec, back))
-    expect = (v1.astype(object) * v2.astype(object)) % P.t
-    assert np.array_equal(vals.astype(object), expect)
+    if P.ctx.using_batching:
+        vals = R.batch_decode(be_, R.decrypt(dec, back))
+        expect = (v1.astype(object) * v2.astype(object)) % P.t
+        assert np.array_equal(vals.astype(object), expect)
+    else:
+        coeffs = R.pt_coeffs(R.decrypt(dec, back))
+        vals = np.zeros(P.n, dtype=np.uint64)
+        vals[: coeffs.size] = coeffs
+        eq(vals, negacyclic_mul_mod(v1, v2, P.t), "decrypted product")
     return dict(dec=dec, sk=sk, ct=got, expect_plain=R.pt_coeffs(R.decrypt(dec, back)))
 
 
@@ -436,3 +461,61 @@ def check_adversarial_keyswitch(P):
         o2 = P.out(2, P.k, P.n)
         P.ctx.apply_galois(P.dev(a), 3, dk, o2, 1)
         eq(P.host(o2), R.ct_words(R.rotate_rows(R.new_ct(a), 1, glk)), "rotate_rows(qm1) with an all-(p-1) key")
+
+
+def check_golden_appendix_b(be, g):
+    """The library on the RNG-free App. B vectors against the unmodified reference's outputs stored in
+    tests/golden/appendix_b.json (FNV-1a-64 of every output word; tests/golden/make_golden.py): no reference library needed."""
+    n, moduli, t = g["n"], g["moduli"], g["t"]
+    ctx = B200Context(n, moduli, t, lib=be.lib)
+    k = ctx.k()
+    assert k == g["k"]
+    c = g["context"]
+    li = ctx.level_info(ctx.first_level)
+    assert li["parms_id"] == c["first_parms_id"] and ctx.level_info(0)["parms_id"] == c["key_parms_id"]
+    assert li["gamma"] == c["gamma"] and li["delta"] == c["delta"]
+    assert li["q_mod_t"] in (c["q_mod_t"] % t, c["q_mod_t"])
+    assert li["roots"] == c["roots"][:k]
+    inp = appendix_b_inputs(n, moduli, t)
+    assert {name: "%016x" % fnv1a64(v) for name, v in inp.items()} == g["inputs"]
+    H = lambda x: "%016x" % fnv1a64(be.to_host(x))
+    a, b, p, rlk = (be.to_dev(inp[x]) for x in ("a", "b", "p", "rlk"))
+    got = {}
+    o2, o3 = be.empty((2, k, n)), be.empty((3, k, n))
+    ctx.add(a, b, o2, 2, 1)
+    got["add"] = H(o2)
+    ctx.sub(a, b, o2, 2, 1)
+    got["sub"] = H(o2)
+    ctx.negate(a, o2, 2, 1)
+    got["negate"] = H(o2)
+    ctx.multiply(a, 2, b, 2, o3, 1)
+    got["multiply"] = H(o3)
+    ctx.relinearize(o3, rlk, o2, 1)
+    got["relinearize"] = H(o2)
+    ctx.multiply_relin(a, b, rlk, o2, 1)
+    got["multiply_relin"] = H(o2)
+    ctx.square(a, o3, 1)
+    got["square"] = H(o3)
+    ctx.multiply_plain(a, 2, p, 1, o2, 1)
+    got["multiply_plain"] = H(o2)
+    ctx.add_plain(a, 2, p, 1, o2, 1)
+    got["add_plain"] = H(o2)
+    ctx.sub_plain(a, 2, p, 1, o2, 1)
+    got["sub_plain"] = H(o2)
+    exp = dict(g["ops"], multiply_relin=g["ops"]["relinearize"])
+    if k >= 2:
+        om = be.empty((2, k - 1, n))
+        ctx.mod_switch_to_next(a, 2, om, 1)
+        got["mod_switch_to_next"] = H(om)
+    if exp["rotate_rows_1"] is not None:
+        assert ctx.galois_elt_from_step(1) == 3 and ctx.galois_elt_from_step(0) == 2 * n - 1
+        ctx.apply_galois(a, 3, be.to_dev(inp["glk3"]), o2, 1)
+        got["rotate_rows_1"] = H(o2)
+        ctx.apply_galois(a, 2 * n - 1, be.to_dev(inp["glkc"]), o2, 1)
+        got["rotate_columns"] = H(o2)
+    else:
+        got["rotate_rows_1"] = got["rotate_columns"] = None
+    x = be.to_dev(inp["a"][0])
+    ctx.ntt_forward(x, 1)
+    got["ntt_a_p0_r0"] = "%016x" % fnv1a64(be.to_host(x)[0])
+    assert got == {name: exp[name] for name in got}, {name: (got[name], exp[name]) for name in got if got[name] != exp[name]}

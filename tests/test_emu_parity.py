@@ -1,17 +1,27 @@
 """CPU-side parity: the product sources compiled in the test-only emulation mode (tests/emu) against the
 unmodified reference, on the RNG-free vectors of SURVEY.md App. B.  Covers host precompute, constant folding,
 strides and the orchestration of every layer-1 entry point; the CUDA build itself is covered by test_gpu_parity."""
+import json
+import os
+
 import pytest
 
 import parity_checks as pc
 from backends import EmuBackend
 from params import PARAMS
 
+GOLD = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "appendix_b.json")))
+
 
 @pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49"])
 def pair(request, emu_lib, ref):
     n, moduli, t = PARAMS[request.param]
     return pc.Pair(EmuBackend(emu_lib), n, moduli, t)
+
+
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_54", "n8192_49"])
+def test_golden_appendix_b(emu_lib, name):
+    pc.check_golden_appendix_b(EmuBackend(emu_lib), GOLD[name])
 
 
 def test_context_constants(pair):
@@ -32,8 +42,6 @@ def test_multiply_and_relinearize(pair):
 
 
 def test_galois(pair):
-    if not pair.ctx.using_batching:
-        pytest.skip("t does not support batching (reference raises logic_error)")
     pc.check_galois(pair)
 
 
@@ -76,8 +84,6 @@ def test_noise_norm(pair):
 
 
 def test_encrypted_roundtrip(pair):
-    if not pair.ctx.using_batching:
-        pytest.skip("needs a batching plain modulus")
     pc.check_encrypted_roundtrip(pair)
 
 

@@ -1,5 +1,5 @@
-// tools/ubench.cu — developer microbenchmarks (not part of the product): integer pipe rates on sm_100a that
-// decide the NTT butterfly design. Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench ubench.cu
+// tools/ubench.cu — developer microbenchmarks (not part of the product): integer pipe rates on sm_90a that
+// decide the NTT butterfly design. Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench ubench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 typedef unsigned long long u64;

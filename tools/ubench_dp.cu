@@ -1,4 +1,4 @@
-// Developer microbenchmark: FP64 pipe throughput on sm_100a as a function of resident warps per SM sub-partition and of
+// Developer microbenchmark: FP64 pipe throughput on sm_90a as a function of resident warps per SM sub-partition and of
 // the number of independent dependency chains per thread (how much parallelism the NTT kernels need to fill the pipe).
 #include <cstdio>
 #include <cuda_runtime.h>
