@@ -194,6 +194,10 @@ void b200_ntt_timeline(b200_ctx *ctx, unsigned long long *device_buffer);
 /* developer aid: select the FP64 NTT kernel variant for subsequent launches (bit 0: twiddle table in shared memory; the
    other bits are timing ablations whose RESULTS ARE MEANINGLESS — tools/ntt_ablate.py); returns the previous value */
 int b200_debug_ntt_variant(int variant);
+/* developer aid: resident CTAs per SM of the FP64 NTT kernel (log2 n, forward != 0, threads per CTA, variant), as the
+   launcher queries it to size the grid of the persistent variant; B200_E_INVALID when that kernel is not instantiated.
+   Meaningful once a context exists (context creation raises the kernels' shared-memory limit) */
+int b200_debug_ntt_ctas_per_sm(int logn, int forward, int threads, int variant);
 /* developer aid: start-up stagger (clock cycles per resident CTA slot) of the streaming NTT kernel; returns the previous value */
 int b200_debug_ntt_stagger(int cycles);
 

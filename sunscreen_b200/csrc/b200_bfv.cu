@@ -2136,6 +2136,23 @@ int b200_debug_ntt_variant(int variant)
     return 0;
 #endif
 }
+int b200_debug_ntt_ctas_per_sm(int logn, int forward, int threads, int variant)
+{
+#ifndef B200_EMU_HEADER
+    // the query launch_ntt makes for the grid of the persistent variant (same kernel, same dynamic shared memory)
+    b200_ntt_fp_fn sfn = b200_ntt_fp_kernel(logn, forward != 0, threads, variant);
+    if (!sfn)
+        return fail(B200_E_INVALID, "no FP64 NTT kernel for this (size, direction, CTA width, variant)");
+    const size_t smem = (size_t)ntt_smem_words(1 << logn) * sizeof(u64) + ((variant & 1) ? B200_NTT_TWS_ENTRIES * sizeof(double) : 0);
+    return b200_ntt_fp_ctas_per_sm(sfn, threads, smem);
+#else
+    (void)logn;
+    (void)forward;
+    (void)threads;
+    (void)variant;
+    return fail(B200_E_INVALID, "the emulation build has no FP64 NTT kernels");
+#endif
+}
 void b200_ntt_timeline(b200_ctx *ctx, unsigned long long *device_buffer)
 {
     if (ctx)

@@ -50,6 +50,7 @@ _SIGS = {
     "b200_memcpy_d2d": [vp, vp, vp, C.c_size_t, vp],
     "b200_memzero": [vp, vp, C.c_size_t, vp],
     "b200_debug_ntt_variant": [C.c_int],
+    "b200_debug_ntt_ctas_per_sm": [C.c_int, C.c_int, C.c_int, C.c_int],
     "b200_debug_ntt_stagger": [C.c_int],
     "b200_gather_scatter_table": [vp, vp, u64, vp, u64, C.c_int, vp],
     "b200_malloc_async": [vp, C.c_size_t, C.POINTER(vp), vp],

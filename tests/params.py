@@ -1,6 +1,7 @@
 """Parameter sets used by the parity tests and bench (SURVEY.md §8(d), BASELINE.json configs).
 Moduli are the reference's BFVDefault tables (S/util/globals.cpp:23-71); t = PlainModulus::Batching(n, 20)
-except n=4096 where Sunscreen's default t = 262144 is used (sunscreen/src/compiler.rs:155)."""
+except n=4096 where Sunscreen's default t = 262144 is used (sunscreen/src/compiler.rs:155).  The edge chains at the end
+come from CoeffModulus::Create instead."""
 
 DEFAULT_MODULI = {
     4096: [0xffffee001, 0xffffc4001, 0x1ffffe0001],
@@ -22,6 +23,41 @@ PARAMS = {
     "n8192_49": (8192, [0xffffffffc001, 0x1fffffff74001, 0x1fffffff68001, 0x1fffffff50001], 1032193),
     "n16384": (16384, DEFAULT_MODULI[16384], 786433),
     "n32768": (32768, DEFAULT_MODULI[32768], 786433),
-    # seal_fhe's own unit-test parameters (seal_fhe/src/bfv_evaluator.rs:305-960): CoeffModulus::Create(8192,{50,30,30,50,50})
-    # is generated by prime search in the reference; kept out of the fixed table on purpose (see test_host_ctx).
 }
+
+# Edge chains: what CoeffModulus::Create(n, bits) returns for each, in its order (same-width primes are handed out
+# smallest first); tests/test_params.py re-derives every list.  Each set reaches kernel choices the homogeneous
+# BFVDefault chains above never make.
+EDGE_BITS = {
+    # seal_fhe's own evaluator tests (seal_fhe/src/bfv_evaluator.rs:305-960): 50-bit primes on the integer path, 30-bit
+    # ones on FP64, so every NTT job is mixed and the BEHZ base is the reference's 61-bit one
+    "n8192_sealfhe": (8192, [50, 30, 30, 50, 50]),
+    # >= 50-bit and 48/49-bit primes in one chain: at logn 14 every transform of a mixed job, FP64-capable primes
+    # included, runs the generic integer kernel, and the BEHZ base is the 61-bit one
+    "n16384_mixed": (16384, [50, 49, 50, 48, 49, 50]),
+    # ~20-bit primes under the 47-bit FP64 auxiliary base, t below all of them
+    "n4096_narrow": (4096, [20, 21, 22]),
+    # a 17-bit data prime below t: no fast plain lift (every q_i > t fails)
+    "n4096_q_below_t": (4096, [17, 30, 30]),
+    # the widest primes SEAL allows (60 bits: the 128-bit lazy sums at their largest), and the first integer width
+    "n8192_60": (8192, [60, 60, 60]),
+    "n8192_50": (8192, [50, 50, 50, 50]),
+    # two-prime chains at logn 11 and 10: key switching with the generic 256-thread kernel (54 bits exceed 128-bit
+    # security at n = 1024, so the reference accepts that one only without a security level: SEC_NONE below)
+    "n2048_2x27": (2048, [27, 27]),
+    "n1024_2x27": (1024, [27, 27]),
+}
+
+PARAMS.update({
+    "n8192_sealfhe": (8192, [0x3ffffffef4001, 0x3ffe8001, 0x3fff4001, 0x3fffffffcc001, 0x3ffffffffc001], 1032193),
+    "n16384_mixed": (16384, [0x3ffffffd20001, 0x1fffffff50001, 0x3ffffffd48001, 0xfffffffd8001, 0x1fffffff68001,
+                             0x3ffffffdf0001], 786433),
+    "n4096_narrow": (4096, [0xfc001, 0x1f6001, 0x3fa001], 40961),
+    "n4096_q_below_t": (4096, [0x1c001, 0x3ffee001, 0x3fff4001], 786433),
+    "n8192_60": (8192, [0xffffffffffd8001, 0xffffffffffe8001, 0xfffffffffffc001], 1032193),
+    "n8192_50": (8192, [0x3ffffffe94001, 0x3ffffffef4001, 0x3fffffffcc001, 0x3ffffffffc001], 1032193),
+    "n2048_2x27": (2048, [0x7fe6001, 0x7ff6001], 12289),
+    "n1024_2x27": (1024, [0x7ffc801, 0x7fff801], 12289),
+})
+SEC_NONE = {"n1024_2x27"}   # sets the reference must be created for without a security level
+EDGE = list(EDGE_BITS)

@@ -8,15 +8,14 @@ import pytest
 
 import parity_checks as pc
 from backends import EmuBackend
-from params import PARAMS
+from params import EDGE, PARAMS
 
 GOLD = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "appendix_b.json")))
 
 
-@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49"])
+@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49"] + EDGE)
 def pair(request, emu_lib, ref):
-    n, moduli, t = PARAMS[request.param]
-    return pc.Pair(EmuBackend(emu_lib), n, moduli, t)
+    return pc.pair_for(EmuBackend(emu_lib), request.param)
 
 
 @pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_54", "n8192_49"])
@@ -151,3 +150,18 @@ def test_layer1_argument_checks(emu_lib):
                      (L.b200_multiply_relin, (h, ci(lv), p, p, p, p, u64(0), None))):
         fn.restype = C.c_int
         assert fn(*args) == 0
+
+
+def test_n8192_with_the_reference_auxiliary_base(emu_lib, ref, monkeypatch):
+    """The all-FP64 default chain with the reference's 61-bit auxiliary base (read when the context is created): the BEHZ
+    jobs then mix FP64 data primes with integer-path auxiliary primes."""
+    monkeypatch.setenv("B200_FORCE_AUX61", "1")
+    P = pc.Pair(EmuBackend(emu_lib), *PARAMS["n8192"])
+    assert P.ctx.level_info(P.ctx.first_level)["m_sk"] == P.ref.rns_info()["m_sk"]
+    pc.check_context(P)
+    pc.check_ntt(P)
+    m3, rm = pc.check_multiply(P)
+    pc.check_relin(P, m3, rm)
+    pc.check_galois(P)
+    pc.check_adversarial_multiply(P, with_size5=False, pairs=[("qm1", "qm1"), ("alt", "pm1")])
+    pc.check_adversarial_keyswitch(P)

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import parity_checks as pc
-from params import PARAMS
+from params import EDGE, PARAMS
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -20,10 +20,9 @@ def be():
     return CudaBackend()
 
 
-@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49", "n16384", "n32768"])
+@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49", "n16384", "n32768"] + EDGE)
 def pair(request, be, ref):
-    n, moduli, t = PARAMS[request.param]
-    return pc.Pair(be, n, moduli, t)
+    return pc.pair_for(be, request.param)
 
 
 @pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_54", "n8192_49", "n16384", "n32768"])
@@ -202,3 +201,26 @@ def test_full_size_properties(be):
     oh = np.zeros((B, 2, k, n), dtype=np.uint64)
     ctx.multiply_relin_host(A, Bc, dK, oh, B)
     pc.eq(oh, got, "multiply_relin_host")
+
+
+@pytest.mark.parametrize("setting", ["B200_FORCE_AUX61", "B200_NO_STATIC_NTT"])
+def test_n8192_through_mixed_job_paths(be, ref, monkeypatch, setting):
+    """The all-FP64 default chain routed through the code that mixed chains take: with the reference's 61-bit auxiliary
+    base every BEHZ job holds integer-path primes (its transforms, FP64-capable primes included, run the generic integer
+    kernel, and the BEHZ / key-switch kernels take their integer variants), and without the static kernel every transform
+    runs the generic integer kernel.  B200_FORCE_AUX61 is read when the context is created; B200_NO_STATIC_NTT then,
+    for the FP64 bound analysis, and again at each transform, so both stay set for the whole check."""
+    monkeypatch.setenv(setting, "1")
+    P = pc.Pair(be, *PARAMS["n8192"])
+    li = P.ctx.level_info(P.ctx.first_level)
+    assert (li["m_sk"] == P.ref.rns_info()["m_sk"]) == (setting == "B200_FORCE_AUX61")
+    pc.check_context(P)
+    pc.check_ntt(P, items=7)
+    m3, rm = pc.check_multiply(P)
+    pc.check_relin(P, m3, rm)
+    pc.check_galois(P)
+    pc.check_plain(P)
+    pc.check_modswitch(P)
+    pc.check_batch(P, batch=5)
+    pc.check_adversarial_multiply(P, with_size5=True)
+    pc.check_adversarial_keyswitch(P)

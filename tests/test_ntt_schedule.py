@@ -5,7 +5,9 @@ instantiated shape without a GPU:
   * after the first forward pass (before the last inverse pass) the groups a warp group handles touch ONLY the elements of that
     group's own block(s), in every remaining pass — which is why a __syncwarp / named barrier of that group is enough between them;
   * the write-out / copy-in of a group covers exactly its block(s).
-The kernel itself is covered bit for bit by the GPU parity tests with every variant forced (B200_NTT_VAR)."""
+The kernels themselves are compared bit for bit with the reference by tests/test_gpu_launch_shapes.py, which forces each
+correct variant (0, 1, 16, 2048, 2049, 2064) of every instantiated shape through b200_debug_ntt_variant; the timing
+ablations are left out."""
 import pytest
 
 SCHED = {12: (4, 4, 4), 13: (3, 3, 3, 4), 14: (3, 3, 4, 4)}   # NttSched<LOGN>: stages per forward pass

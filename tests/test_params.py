@@ -1,0 +1,105 @@
+"""The parameter table itself: every chain is a list of distinct primes = 1 mod 2n, and each edge chain is exactly what
+CoeffModulus::Create(n, bits) returns (the reference's prime search, restated here; compared with the reference library
+itself where it is built)."""
+import ctypes as C
+
+import pytest
+
+from params import EDGE, EDGE_BITS, PARAMS, SEC_NONE
+
+
+def is_prime(v):
+    """Deterministic Miller-Rabin for v < 2^64."""
+    if v < 2:
+        return False
+    bases = (2, 3, 5, 7, 11, 13, 17, 19, 23, 29, 31, 37)
+    for p in bases:
+        if v % p == 0:
+            return v == p
+    d, s = v - 1, 0
+    while d % 2 == 0:
+        d, s = d // 2, s + 1
+    for a in bases:
+        x = pow(a, d, v)
+        if x in (1, v - 1):
+            continue
+        for _ in range(s - 1):
+            x = x * x % v
+            if x == v - 1:
+                break
+        else:
+            return False
+    return True
+
+
+def create_coeff_modulus(n, bit_sizes):
+    """CoeffModulus::Create: per width, the `count` largest primes = 1 mod 2n below 2^width, descending; the requested
+    widths are then served in order, each taking the SMALLEST prime left of its width."""
+    table = {}
+    for bits in set(bit_sizes):
+        count, found = bit_sizes.count(bits), []
+        v = ((1 << bits) - 1) // (2 * n) * (2 * n) + 1
+        while count and v > 1 << (bits - 1):
+            if is_prime(v):
+                found.append(v)
+                count -= 1
+            v -= 2 * n
+        table[bits] = found
+    return [table[bits].pop() for bits in bit_sizes]
+
+
+@pytest.mark.parametrize("name", sorted(PARAMS))
+def test_chain_primes(name):
+    n, moduli, t = PARAMS[name]
+    assert len(set(moduli)) == len(moduli) >= 2
+    for q in moduli:
+        assert is_prime(q) and q % (2 * n) == 1 and q.bit_length() <= 60, hex(q)
+    assert t < 1 << 60 and t not in moduli
+
+
+@pytest.mark.parametrize("name", EDGE)
+def test_edge_chain_is_create_output(name):
+    n, bits = EDGE_BITS[name]
+    _, moduli, _ = PARAMS[name]
+    assert [q.bit_length() for q in moduli] == bits
+    assert moduli == create_coeff_modulus(n, bits)
+
+
+def test_edge_chains_reach_their_cases():
+    """What each edge chain is there for (host_ctx.cpp: FP64 primes are <= 49 bits; fast plain lift needs every data prime
+    above t; batching needs t prime and = 1 mod 2n)."""
+    fp = lambda q: q.bit_length() <= 49
+    n, m, t = PARAMS["n8192_sealfhe"]
+    assert t == 1032193 and any(map(fp, m)) and not all(map(fp, m))
+    n, m, t = PARAMS["n16384_mixed"]
+    assert {q.bit_length() for q in m[:-1]} >= {48, 49, 50}
+    n, m, t = PARAMS["n4096_narrow"]
+    assert all(q.bit_length() <= 22 for q in m) and t < min(m) and is_prime(t) and t % (2 * n) == 1
+    n, m, t = PARAMS["n4096_q_below_t"]
+    assert min(m[:-1]) < t < max(m[:-1]) and is_prime(t) and t % (2 * n) == 1
+    assert all(q.bit_length() == 60 for q in PARAMS["n8192_60"][1])
+    assert all(q.bit_length() == 50 for q in PARAMS["n8192_50"][1])
+    for name, logn in (("n2048_2x27", 11), ("n1024_2x27", 10)):
+        n, m, t = PARAMS[name]
+        assert n == 1 << logn and len(m) == 2 and t % (2 * n) == 1
+
+
+@pytest.mark.parametrize("name", EDGE)
+def test_edge_chain_matches_reference_create(ref, name):
+    import refseal
+    n, bits = EDGE_BITS[name]
+    arr = (C.c_int * len(bits))(*bits)
+    out = (C.c_void_p * len(bits))()
+    ref.call("CoeffModulus_Create1", C.c_uint64(n), C.c_uint64(len(bits)), arr, out)
+    got = []
+    for h in out:
+        v = C.c_uint64()
+        ref.call("Modulus_Value", C.c_void_p(h), C.byref(v))
+        got.append(v.value)
+    assert got == PARAMS[name][1]
+    # and the reference accepts the whole set, at 128-bit security unless the set is marked otherwise
+    sec = refseal.SEC_NONE if name in SEC_NONE else refseal.SEC_TC128
+    refseal.RefContext(n, PARAMS[name][1], PARAMS[name][2], sec)
+    if name in SEC_NONE:
+        with pytest.raises(ValueError):
+            refseal.RefContext(n, PARAMS[name][1], PARAMS[name][2])

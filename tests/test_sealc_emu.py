@@ -72,7 +72,7 @@ def test_single_prime_chain(S, ref, n, moduli, t):
     sc.single_prime_context(S, n, moduli, t)
 
 
-@pytest.mark.parametrize("name", ["n4096", "n8192"])
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_sealfhe", "n4096_q_below_t"])
 def test_whole_chain_and_large_sizes(S, ref, name):
     sc.deep_chain_parity(S, *PARAMS[name])
 
@@ -103,7 +103,7 @@ def test_wire_fuzz(S, ref):
     sc.wire_fuzz(S, *PARAMS["n4096"])
 
 
-@pytest.mark.parametrize("name", ["n4096", "n8192"])
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_sealfhe"])
 def test_key_level_order(S, ref, name):
     sc.key_level_order(S, *PARAMS[name])
 

@@ -145,7 +145,7 @@ def test_single_prime_chain(S, ref, n, moduli, t):
     sc.single_prime_context(S, n, moduli, t)
 
 
-@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_49", "n16384"])
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_49", "n16384", "n8192_sealfhe", "n16384_mixed"])
 def test_whole_chain_and_large_sizes(S, ref, name):
     sc.deep_chain_parity(S, *PARAMS[name])
 
@@ -171,7 +171,7 @@ def test_handle_lifetime_order(S, ref):
     sc.handle_lifetime_order(S, *PARAMS["n4096"])
 
 
-@pytest.mark.parametrize("name", ["n4096", "n8192", "n16384"])
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n16384", "n8192_sealfhe", "n16384_mixed"])
 def test_key_level_order(S, ref, name):
     sc.key_level_order(S, *PARAMS[name])
 
