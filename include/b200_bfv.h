@@ -119,7 +119,10 @@ int b200_multiply_relin(b200_ctx *ctx, int level, const uint64_t *a, const uint6
 /* size-2 cts: out = (sigma_g(c0), 0) + KeySwitch(sigma_g(c1), galois_key) */
 int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
                       uint64_t *out2, uint64_t batch, void *stream);
-/* plain: [batch or 1][n] coefficients mod t (plain_batch = 1 broadcasts one plaintext to every item) */
+/* plain: [batch or 1][n] coefficients mod t (plain_batch = 1 broadcasts one plaintext to every item).  multiply_plain
+   follows the reference per plaintext item: an item with exactly one nonzero coefficient m is multiplied by m itself
+   (its monomial path); any other item, and a monomial item when some q_i <= t, by the lifted plaintext
+   (m + (Q - t) for m >= (t+1)/2).  The two are congruent mod t but give different ciphertext words. */
 int b200_multiply_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t plain_batch,
                         uint64_t *out, uint64_t batch, void *stream);
 int b200_add_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t plain_batch,

@@ -550,7 +550,50 @@ __global__ void dyadic_plain_kernel(const PrimeDev *primes, int k, int size, con
     out[idx] = barrett128(lo, hi, P.p, P.r0, P.r1);
 }
 
-__global__ void plain_lift_kernel(const LevelDev L, const u64 *plain, u64 *out, int logn, long long total)
+// mono[item] = 1 when plaintext `item` has exactly one nonzero coefficient (the monomial test of multiply_plain_normal,
+// S/evaluator.cpp:1885).  One block per item: strided per-thread counts, summed in shared memory (blockDim a power of 2).
+// The CPU emulation build runs kernels with dynamic shared memory as one thread per block, so only the CUDA build executes
+// the tree reduction; the GPU parity tests (check_plain_operands, batches of monomial and dense items) cover it.
+__global__ void plain_monomial_kernel(const u64 *plain, long long n, u32 *mono)
+{
+#ifdef B200_EMU_HEADER
+    u64 *sm = (u64 *)emu_shared;
+#else
+    extern __shared__ u64 sm[];
+#endif
+    const u64 *p = plain + (long long)blockIdx.x * n;
+    u64 cnt = 0;
+    // four independent loads in flight per step; a thread that has seen two nonzero coefficients has decided that the item
+    // is no monomial and stops, so a dense plaintext costs one step
+    for (long long c = threadIdx.x; c < n && cnt < 2; c += 4LL * blockDim.x)
+    {
+        u64 v[4];
+#pragma unroll
+        for (int u = 0; u < 4; u++)
+        {
+            const long long i = c + (long long)u * blockDim.x;
+            v[u] = i < n ? p[i] : 0;
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++)
+            cnt += v[u] != 0;
+    }
+    sm[threadIdx.x] = cnt;
+    B200_SYNC();
+    for (int s = (int)blockDim.x >> 1; s > 0; s >>= 1)
+    {
+        if ((int)threadIdx.x < s)
+            sm[threadIdx.x] += sm[threadIdx.x + s];
+        B200_SYNC();
+    }
+    if (threadIdx.x == 0)
+        mono[blockIdx.x] = sm[0] == 1;
+}
+
+// mono: per-item flags of plain_monomial_kernel, or null.  A monomial item is multiplied by its coefficient itself, the
+// reference's monomial path (S/evaluator.cpp:1885-1933); the flags are only passed under the fast plain lift, where that
+// differs from the general lift for a coefficient at or above the threshold (m instead of m + q_i - t).
+__global__ void plain_lift_kernel(const LevelDev L, const u64 *plain, const u32 *mono, u64 *out, int logn, long long total)
 {
     const long long idx = GLOBAL_IDX();
     if (idx >= total)
@@ -561,7 +604,8 @@ __global__ void plain_lift_kernel(const LevelDev L, const u64 *plain, u64 *out, 
     const int r = (int)(t % L.k);
     const long long item = t / L.k;
     const PrimeDev Q = ld_prime(&L.q[r]);
-    out[idx] = plain_lift(L, Q, r, plain[item * n + c]);
+    const u64 m = plain[item * n + c];
+    out[idx] = mono && mono[item] ? barrett64(m, Q.p, Q.r1) : plain_lift(L, Q, r, m);
 }
 
 // c0 +/- scaled plaintext; other polys copied.  sign: 0 add, 1 sub
@@ -1064,6 +1108,7 @@ static int build_device(b200_ctx *ctx)
         UPF(plain_inc, Lh.plain_upper_half_inc);
         L.q_mod_t = Lh.q_mod_t;
         L.plain_thr = Lh.plain_upper_half_threshold;
+        L.fast_plain_lift = Lh.fast_plain_lift ? 1 : 0;
         LevelFpHost fp_level;
         {
             bool lfp = ctx->fp_enabled && H.aux_bits <= b200::FP_PRIME_BITS;
@@ -2614,9 +2659,20 @@ int b200_multiply_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, c
     u64 *pl = nullptr;
     if ((rc = scr.get((size_t)pb * k * n, &pl)))
         return rc;
+    u32 *mono = nullptr;
+    if (L.fast_plain_lift)
+    {
+        u64 *flags = nullptr;
+        if ((rc = scr.get((size_t)(pb + 1) / 2, &flags)))
+            return rc;
+        mono = (u32 *)flags;
+        B200_LAUNCH(plain_monomial_kernel, (unsigned)pb, 1024, 1024 * sizeof(u64), s, (const u64 *)plain, n, mono);
+        ctx->launches++;
+    }
     {
         const long long total = (long long)pb * k * n;
-        B200_LAUNCH(plain_lift_kernel, blocks_for(total, EB), EB, 0, s, L, (const u64 *)plain, pl, ctx->logn, total);
+        B200_LAUNCH(plain_lift_kernel, blocks_for(total, EB), EB, 0, s, L, (const u64 *)plain, (const u32 *)mono, pl, ctx->logn,
+                                                                total);
         ctx->launches++;
     }
     JobDesc jd;

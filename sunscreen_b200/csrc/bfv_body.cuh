@@ -55,6 +55,7 @@ struct LevelDev
     const u64 *delta;      // [k]
     const u64 *plain_inc;  // [k]
     u64 q_mod_t, plain_thr;
+    int fast_plain_lift;   // every q_i > t (ContextData::qualifiers().using_fast_plain_lift)
     // FP64 fast path (every prime of the level and of the aux base is below 2^47): the same constants as
     // integer-valued doubles, each entry {w, w/p_target}; primes as {p, 1/p}
     int fp;

@@ -61,3 +61,30 @@ PARAMS.update({
 })
 SEC_NONE = {"n1024_2x27"}   # sets the reference must be created for without a security level
 EDGE = list(EDGE_BITS)
+
+# Plain moduli beyond 20 bits on chains above: name -> (chain, how t is chosen).  A batching t is what
+# PlainModulus::Batching(n, bits) returns, the largest prime = 1 mod 2n below 2^bits (CoeffModulus::Create(n, {bits})),
+# skipping the chain's own primes where noted; tests/test_params.py re-derives each.
+PLAIN_EDGE_T = {
+    "n4096_t2": ("n4096", 2),                       # the smallest t: threshold 1, every nonzero coefficient is upper half
+    "n4096_t2p40": ("n4096", 1 << 40),              # a 41-bit power of two, not batching
+    "n8192_t30": ("n8192", ("batching", 30)),
+    "n8192_t49": ("n8192", ("batching", 49)),       # the FP64 plain NTT at its width limit
+    "n8192_t47": ("n8192", ("batching", 47)),       # = the first 47-bit FP64 auxiliary candidate, which must be skipped
+    "n8192_t3p37": ("n8192", 3 ** 37),              # odd composite, 59 bits
+    "n8192_54_t60": ("n8192_54", ("batching", 60)),  # 32 + 60 + bits(Q) >= 61 (k + 1): the reference's nB = k + 1
+    "n8192_60_t60": ("n8192_60", ("batching", 60)),  # the largest 60-bit batching prime is in the chain: the next one
+    "n16384_t60": ("n16384", ("batching", 60)),     # the 49-bit FP64 auxiliary base less than one prime above its range bound
+}
+PARAMS.update({
+    "n4096_t2": (4096, DEFAULT_MODULI[4096], 2),
+    "n4096_t2p40": (4096, DEFAULT_MODULI[4096], 1 << 40),
+    "n8192_t30": (8192, DEFAULT_MODULI[8192], 0x3fff4001),
+    "n8192_t49": (8192, DEFAULT_MODULI[8192], 0x1fffffff74001),
+    "n8192_t47": (8192, DEFAULT_MODULI[8192], 0x7ffffffec001),
+    "n8192_t3p37": (8192, DEFAULT_MODULI[8192], 3 ** 37),
+    "n8192_54_t60": (8192, PARAMS["n8192_54"][1], 0xfffffffffffc001),
+    "n8192_60_t60": (8192, PARAMS["n8192_60"][1], 0xffffffffffc4001),
+    "n16384_t60": (16384, DEFAULT_MODULI[16384], 0xffffffffffe8001),
+})
+PLAIN_EDGE = list(PLAIN_EDGE_T)

@@ -3,7 +3,7 @@ import math
 
 import numpy as np
 
-from refseal import E_INVALIDARG, SEC_TC128, RefContext, SealError, appendix_b_inputs, fnv1a64
+from refseal import COR_E_INVALIDOPERATION, E_INVALIDARG, SEC_TC128, RefContext, SealError, appendix_b_inputs, fnv1a64
 from sunscreen_b200.lib import B200Context
 
 
@@ -68,8 +68,11 @@ def check_context(P):
     assert P.ctx.level_info(0)["parms_id"] == list(P.ref.key_parms_id)
     assert li["gamma"] == ri["gamma"]
     if li["m_sk"] == ri["m_sk"]:
-        # the reference's own auxiliary base (61-bit primes)
+        # the reference's own auxiliary base (61-bit primes), |B| = k, plus one when 32 + bits(t) + bits(Q) >= 61 (k + 1)
+        # (S/util/rns.cpp:617-624)
         assert li["bsk"] == ri["bsk_primes"] and (li["nB"], li["nBsk"]) == (ri["B"], ri["Bsk"])
+        Q = math.prod(li["q"])
+        assert li["nB"] == li["k"] + (32 + P.t.bit_length() + Q.bit_length() >= 61 * li["k"] + 61)
     else:
         # FP64-friendly auxiliary base: 47..49-bit NTT primes (as wide as the widest user prime), distinct from the user's
         # primes, with at least the reference's dynamic range condition
@@ -77,7 +80,7 @@ def check_context(P):
         width = max(47, max(int(m).bit_length() for m in P.moduli))
         assert width <= 49
         assert all(p < (1 << width) and p % (2 * P.n) == 1 for p in li["bsk"]) and len(set(li["bsk"])) == len(li["bsk"])
-        assert not set(li["bsk"]) & set(int(m) for m in P.moduli)
+        assert not set(li["bsk"]) & set(int(m) for m in P.moduli) and P.t not in li["bsk"]
         Q = math.prod(li["q"])
         assert math.prod(li["bsk"]).bit_length() > 32 + P.t.bit_length() + Q.bit_length()
     pi = P.ref.plain_info()
@@ -211,10 +214,83 @@ def check_plain(P):
     eq(P.host(o2), P.ref.ct_words(P.ref.sub_plain(ra, rp)), "sub_plain")
     # monomial plaintext (the reference takes its fast path, S/evaluator.cpp:1885-1933): same words expected
     mono = np.zeros(P.n, dtype=np.uint64)
-    mono[5] = 7
+    mono[5] = 7 if 7 < (P.t + 1) // 2 else 1
     rm = P.ref.new_pt(mono[:6])
     P.ctx.multiply_plain(da, 2, P.dev(mono), 1, o2, 1)
     eq(P.host(o2), P.ref.ct_words(P.ref.multiply_plain(ra, rm)), "multiply_plain(monomial)")
+
+
+def plain_operand_classes(n, t, rng):
+    """(label, coefficients) of the plaintexts whose lift differs between the reference's paths: monomials m * x^e with m in
+    {1, thr - 1, thr, t - 1, t, t + 5} (thr = (t+1)/2, the upper-half threshold; the Evaluator checks only metadata, so
+    coefficients >= t are defined) at e in {0, 1, n - 1}; dense plaintexts in the upper half and in [t, t + 5]; and two
+    nonzero coefficients, just off the monomial path.  Shuffled, so monomial and dense items alternate within a batch."""
+    thr = (t + 1) // 2
+    out = []
+    for m in sorted({1, thr - 1, thr, t - 1, t, t + 5} - {0}):
+        for e in (0, 1, n - 1):
+            p = np.zeros(n, dtype=np.uint64)
+            p[e] = m
+            out.append((f"{m} * x^{e}", p))
+    out.append(("dense upper half", rng.integers(thr, t, size=n, dtype=np.uint64)))
+    out.append(("dense in [t, t + 5]", rng.integers(t, t + 6, size=n, dtype=np.uint64)))
+    two = np.zeros(n, dtype=np.uint64)
+    two[3], two[n - 1] = t - 1, thr
+    out.append(("two nonzero", two))
+    return [out[i] for i in rng.permutation(len(out))]
+
+
+def check_plain_operands(P, seed=41):
+    """multiply_plain / add_plain / sub_plain with every plaintext class of plain_operand_classes, one per item of a batch
+    (plain_batch == batch, so the monomial test is per item), at every data level of the reference's chain through
+    layer 1's `level` argument, word for word against the reference's Evaluator; then one monomial broadcast to every item
+    (plain_batch = 1).  Where the reference's product is transparent (a monomial t under a prime below t: Q - t + t = Q),
+    it refuses it and the layer-1 words must be all zero."""
+    rng = np.random.default_rng(seed)
+    R = P.ref
+    classes = plain_operand_classes(P.n, P.t, rng)
+    labels = [c[0] for c in classes]
+    plains = np.stack([c[1] for c in classes])
+    B = len(classes)
+    dpl = P.dev(plains)
+    thr = (P.t + 1) // 2
+    minus_one = np.zeros((1, P.n), dtype=np.uint64)
+    minus_one[0, 0] = P.t - 1
+    rpls = [R.new_pt(p) for p in plains]
+    rp = R.new_pt(minus_one[0, :1])
+    for j in range(len(R.data_parms_ids())):
+        lv = P.ctx.first_level + j
+        k = P.ctx.level_info(lv)["k"]
+        assert k == R.k - j
+        moduli = P.moduli[:k]
+        cts = rand_ct(rng, moduli, k, P.n, batch=B)
+        dct = P.dev(cts)
+        out = P.out(B, 2, k, P.n)
+        rcts = [R.new_ct(cts[i], level=j) for i in range(B)]
+        for op in ("multiply_plain", "add_plain", "sub_plain"):
+            getattr(P.ctx, op)(dct, 2, dpl, B, out, B, level=lv)
+            got = P.host(out).reshape(B, 2, k, P.n)
+            for i in range(B):
+                try:
+                    rr = getattr(R, op)(rcts[i], rpls[i])
+                except SealError as e:
+                    assert op == "multiply_plain" and e.code == COR_E_INVALIDOPERATION, (op, labels[i], e)
+                    eq(got[i], np.zeros_like(got[i]), f"{op} at level {lv}, item {i} ({labels[i]}): transparent")
+                    continue
+                eq(got[i], R.ct_words(rr), f"{op} at level {lv}, item {i} ({labels[i]})")
+                R.free_ct(rr)
+        # one plaintext for every item: the constant -1 (t - 1 >= thr whenever t > 1)
+        assert P.t - 1 >= thr
+        P.ctx.multiply_plain(dct, 2, P.dev(minus_one), 1, out, B, level=lv)
+        got = P.host(out).reshape(B, 2, k, P.n)
+        for i in range(B):
+            rr = R.multiply_plain(rcts[i], rp)
+            eq(got[i], R.ct_words(rr), f"multiply_plain by (t-1) * x^0 broadcast, level {lv}, item {i}")
+            R.free_ct(rr)
+        for h in rcts:
+            R.free_ct(h)
+    for h in rpls + [rp]:
+        R.free_pt(h)
 
 
 def check_modswitch(P):
@@ -274,11 +350,17 @@ def check_batch(P, batch=3, seed=7):
 
 
 def negacyclic_mul_mod(x, y, t):
-    """x * y in Z_t[X] / (X^n + 1), coefficients of x, y below t < 2^20 (exact in int64 for n <= 32768)."""
+    """x * y in Z_t[X] / (X^n + 1), coefficients of x, y below t < 2^60: the 20-bit limbs are convolved exactly in int64
+    (sums below 2^55 for n <= 32768) and recombined with Python integers."""
     n = x.size
-    c = np.convolve(x.astype(np.int64), y.astype(np.int64))
-    c = np.concatenate([c, np.zeros(1, dtype=np.int64)])
-    return ((c[:n] % t - c[n:] % t) % t).astype(np.uint64)
+    limbs = lambda v: [((v >> np.uint64(20 * i)) & np.uint64(0xFFFFF)).astype(np.int64) for i in range(3)]
+    X, Y = limbs(x), limbs(y)
+    c = np.zeros(2 * n, dtype=object)
+    for i in range(3):
+        for j in range(3):
+            if X[i].any() and Y[j].any():
+                c[: 2 * n - 1] += np.convolve(X[i], Y[j]).astype(object) * (1 << (20 * (i + j)))
+    return ((c[:n] - c[n:]) % t).astype(np.uint64)
 
 
 def check_encrypted_roundtrip(P, seed=3):
@@ -351,10 +433,39 @@ def check_small_kernels(P, seed=29):
         eq(got[:, i, :], want, f"expand_signed residue {i}")
 
 
+def independent_phase(P, ct, powers):
+    """c0 + sum_j c_j * s^j in coefficient form for one ciphertext ct [size][k][n] and NTT-form key powers [size-1][k][n]:
+    the reference's util-level NTT (S/util/ntt.cpp) and dyadic products with Python integers."""
+    size, k = ct.shape[0], ct.shape[1]
+    out = np.empty((k, P.n), dtype=np.uint64)
+    for i in range(k):
+        q = int(P.moduli[i])
+        acc = np.zeros(P.n, dtype=object)
+        for j in range(1, size):
+            acc = (acc + P.ref.ref.ntt_forward(q, ct[j, i]).astype(object) * powers[j - 1, i].astype(object)) % q
+        back = P.ref.ref.ntt_inverse(q, acc.astype(np.uint64))
+        out[i] = ((back.astype(object) + ct[0, i].astype(object)) % q).astype(np.uint64)
+    return out
+
+
+def key_powers(P, s_ntt, k, count):
+    """[count][k][n] NTT-form powers s, s^2, ... of the NTT-form key residues s_ntt [>= k][n], with Python integers."""
+    out = np.empty((count, k, P.n), dtype=np.uint64)
+    for i in range(k):
+        q = int(P.moduli[i])
+        s = s_ntt[i].astype(object)
+        cur = s
+        for j in range(count):
+            out[j, i] = cur.astype(np.uint64)
+            cur = cur * s % q
+    return out
+
+
 def check_noise_norm(P, batch=3, seed=23):
     """b200_noise_norm (the quantity behind invariant_noise_budget, S/decryptor.cpp:424-485): for random ciphertexts of
     size 2 and 3 and random key powers, the device's multi-precision infinity norm of the centred t * phase mod Q equals
-    the same computed with Python integers from the phase words."""
+    the same computed with Python integers from a phase computed independently of the library (independent_phase); the
+    library's own b200_ct_sk_phase must equal that phase too."""
     from functools import reduce
     rng = np.random.default_rng(seed)
     q = [int(m) for m in P.moduli[: P.k]]
@@ -366,7 +477,8 @@ def check_noise_norm(P, batch=3, seed=23):
         dct, dsk = P.dev(ct), P.dev(skp)
         ph = P.out(batch, P.k, P.n)
         P.ctx.ct_sk_phase(dct, size, dsk, ph, batch)
-        phase = P.host(ph).reshape(batch, P.k, P.n)
+        phase = np.stack([independent_phase(P, ct[b], skp) for b in range(batch)])
+        eq(P.host(ph), phase, f"ct_sk_phase, size {size}")
         got = np.zeros((batch, words), dtype=np.uint64)
         P.ctx.noise_norm(dct, size, dsk, got, words, batch)
         coef = [(Q // qi) * pow(Q // qi, -1, qi) * P.t % Q for qi in q]
@@ -378,6 +490,138 @@ def check_noise_norm(P, batch=3, seed=23):
                 best = max(best, v)
             mine = sum(int(got[b, w]) << (64 * w) for w in range(words))
             assert mine == best, f"noise norm, size {size}, item {b}: {mine:#x} != {best:#x}"
+
+
+def decrypt_branch(X, q, t, g):
+    """(upper, zero) for a phase X mod Q = prod(q): whether the {t, gamma} correction of RNSTool::decrypt_scale_and_round
+    (S/util/rns.cpp:1145-1213) takes its vg > gamma/2 branch, and whether the corrected value is 0 (the multiplication by
+    gamma^-1 mod t is then skipped).  Used only to show that the crafted inputs reach every case, never as an expected value."""
+    Q = math.prod(q)
+    s = sum(X * t * g % qi * pow(Q // qi, -1, qi) % qi * (Q // qi) for qi in q)
+    vt = s * -pow(Q, -1, t) % t
+    vg = s * -pow(Q, -1, g) % g
+    upper = vg > g >> 1
+    return upper, ((vt + g - vg) if upper else (vt - vg)) % t == 0
+
+
+def crafted_phases(Q, t, rng):
+    """Phases at the edges of decryption: 0, 1, Q - 1, (Q -+ 1)/2; floor(jQ/t) + {-1, 0, 1} and the rounding boundaries
+    floor((2j+1)Q/(2t)) + {-1, 0, 1, 2} for j in {0, 1, t/2, t - 1} and three random j."""
+    js = {0, 1, t // 2, t - 1} | {int(rng.integers(0, t)) for _ in range(3)}
+    X = [0, 1, Q - 1, (Q - 1) // 2, (Q + 1) // 2]
+    for j in sorted(js):
+        X += [j * Q // t + d for d in (-1, 0, 1)]
+        X += [(2 * j + 1) * Q // (2 * t) + d for d in (-1, 0, 1, 2)]
+    return [x % Q for x in X]
+
+
+def _residues(X, q, n, rng):
+    """[k][n] residues of the integers X (then uniformly random integers below prod(q) to fill n coefficients)."""
+    import random
+    Q = math.prod(q)
+    fill = random.Random(int(rng.integers(0, 2**63)))
+    X = list(X) + [fill.randrange(Q) for _ in range(n - len(X))]
+    return np.array([[x % qi for x in X] for qi in q], dtype=np.uint64), X
+
+
+def check_decrypt(P, batch=5, seed=31):
+    """b200_ct_sk_phase and b200_decrypt at every data level of the reference's chain, with a real reference secret key
+    (its NTT-form words; the powers s^2, s^3 come from Python integers):
+    - uniformly random ciphertexts of size 2, 3 and 4, batch 5: the phase against independent_phase, the plaintext against
+      the reference's Decryptor::decrypt (which accepts any ciphertext);
+    - crafted phases (c1 = 0, so the phase is c0, set by CRT to chosen integers: crafted_phases): the plaintext against the
+      reference's Decryptor and the plain-C oracle's decrypt; the inputs must reach both branches of the gamma correction
+      and its m == 0 skip."""
+    import ctypes as C
+    from oracle_port import OraclePort
+    rng = np.random.default_rng(seed)
+    R = P.ref
+    kg = R.keygen()
+    sk = R.secret_key(kg)
+    dec = R.decryptor(sk)
+    h = C.c_void_p()
+    R.ref.call("SecretKey_Data", sk, C.byref(h))
+    s_ntt = R.pt_coeffs(h).reshape(-1, P.n)
+    gamma = R.rns_info()["gamma"]
+    port = OraclePort().context(P.n, P.moduli, P.t)
+
+    def ref_decrypt(ct, j):
+        c = R.new_ct(ct, level=j)
+        got = R.pt_coeffs(R.decrypt(dec, c))
+        R.free_ct(c)
+        out = np.zeros(P.n, dtype=np.uint64)
+        out[: got.size] = got
+        return out
+
+    for j in range(len(R.data_parms_ids())):
+        lv = P.ctx.first_level + j
+        k = R.k - j
+        assert P.ctx.level_info(lv)["k"] == k
+        pows = key_powers(P, s_ntt, k, 3)
+        dsk = P.dev(pows)
+        for size in (2, 3, 4):
+            ct = rand_ct(rng, P.moduli, k, P.n, size=size, batch=batch)
+            dct = P.dev(ct)
+            ph, pt = P.out(batch, k, P.n), P.out(batch, P.n)
+            P.ctx.ct_sk_phase(dct, size, dsk, ph, batch, level=lv)
+            P.ctx.decrypt(dct, size, dsk, pt, batch, level=lv)
+            gph, gpt = P.host(ph).reshape(batch, k, P.n), P.host(pt).reshape(batch, P.n)
+            for b in range(batch):
+                eq(gph[b], independent_phase(P, ct[b], pows), f"ct_sk_phase, level {lv}, size {size}, item {b}")
+                eq(gpt[b], ref_decrypt(ct[b], j), f"decrypt, level {lv}, size {size}, item {b}")
+        q = [int(m) for m in P.moduli[:k]]
+        Q = math.prod(q)
+        X = crafted_phases(Q, P.t, rng)
+        c0, _ = _residues(X, q, P.n, rng)
+        ct = np.zeros((2, k, P.n), dtype=np.uint64)
+        ct[0] = c0
+        pt = P.out(P.n)
+        P.ctx.decrypt(P.dev(ct), 2, dsk, pt, 1, level=lv)
+        got = P.host(pt).reshape(P.n)
+        eq(got, ref_decrypt(ct, j), f"decrypt of crafted phases, level {lv}")
+        orc = np.zeros(P.n, dtype=np.uint64)
+        assert port.L.orc_decrypt(C.byref(port.c), k, ct.ctypes.data_as(C.c_void_p), 2, np.ascontiguousarray(pows[0]).ctypes.data_as(C.c_void_p),
+                                  orc.ctypes.data_as(C.c_void_p)) == 0
+        eq(got, orc, f"decrypt of crafted phases against the oracle, level {lv}")
+        cases = {decrypt_branch(x, q, P.t, gamma) for x in X}
+        assert {u for u, _ in cases} == {True, False} and {z for _, z in cases} == {True, False}, cases
+
+
+def check_noise_norm_edges(P, seed=37):
+    """b200_noise_norm where its multi-precision arithmetic has edges: phases X with t X = Y (mod Q) for Y = 0, (Q -+ 1)/2
+    (the centring boundary), Q - 1, 2^64 - 1 and 2^64 (a word carry), placed at coefficient 0, 127, 128 (a block boundary)
+    or n - 1 over values below 2^20, in batches of five items, one of them all zero.  Each edge value is the item's largest
+    centred value except Q - 1, whose centred value is 1; the expected norm is computed with Python integers.  `words` above W + 1 leaves the extra words zero; below W + 1 is refused."""
+    rng = np.random.default_rng(seed)
+    q = [int(m) for m in P.moduli[: P.k]]
+    Q = math.prod(q)
+    W = (Q.bit_length() + 63) // 64
+    tinv = pow(P.t, -1, Q)
+    edges = [y for y in ((Q - 1) // 2, (Q + 1) // 2, Q - 1, 2**64 - 1, 2**64) if 0 < y < Q]
+    skp = np.zeros((1, P.k, P.n), dtype=np.uint64)  # c1 = 0: the key powers do not matter
+    dsk = P.dev(skp)
+    centred = lambda y: Q - y if y >= (Q + 1) // 2 else y
+    for p, pos in enumerate((0, 127, 128, P.n - 1)):
+        ct = np.zeros((5, 2, P.k, P.n), dtype=np.uint64)
+        want = [0]
+        for b in range(1, 5):
+            Y = [int(v) for v in rng.integers(0, 2**20, size=P.n)]
+            Y[pos] = edges[(p + b) % len(edges)]
+            want.append(max(centred(y) for y in Y))
+            ct[b, 0], _ = _residues([y * tinv % Q for y in Y], q, P.n, rng)
+        dct = P.dev(ct)
+        for words in (W + 1, W + 3):
+            got = np.zeros((5, words), dtype=np.uint64)
+            P.ctx.noise_norm(dct, 2, dsk, got, words, 5)
+            for b in range(5):
+                mine = sum(int(got[b, w]) << (64 * w) for w in range(words))
+                assert mine == want[b], f"noise norm, maximum at {pos}, item {b}, {words} words: {mine:#x} != {want[b]:#x}"
+    try:
+        P.ctx.noise_norm(dct, 2, dsk, np.zeros((5, W), dtype=np.uint64), W, 5)
+    except Exception as e:  # B200Error(B200_E_INVALID)
+        assert getattr(e, "code", None) == -1, e
+    else:
+        raise AssertionError(f"noise_norm must refuse {W} words for a {Q.bit_length()}-bit modulus")
 
 
 def check_host_pipeline(P, batch=5, seed=17):

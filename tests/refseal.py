@@ -204,16 +204,36 @@ class RefContext:
             out.append(v.value)
         return out
 
+    def data_parms_ids(self):
+        """parms_id of every data level, the first data level first (its own chain: it ends before a modulus below t)."""
+        R = self.ref
+        out = []
+        cd = vp()
+        R.call("SEALContext_FirstContextData", self.ctx, C.byref(cd))
+        while cd.value:
+            parms = vp()
+            R.call("ContextData_Parms", cd, C.byref(parms))
+            pid = (u64 * 4)()
+            R.call("EncParams_GetParmsId", parms, pid)
+            R.call("EncParams_Destroy", parms)
+            out.append(pid)
+            nxt = vp()
+            R.call("ContextData_NextContextData", cd, C.byref(nxt))
+            cd = nxt
+        return out
+
     # ---- data objects ----
-    def new_ct(self, words=None, ntt=False):
-        """words: (size, k, n) uint64 at data level (first_parms_id), or None for an empty destination."""
+    def new_ct(self, words=None, ntt=False, level=0):
+        """words: (size, k, n) uint64 at data level `level` (0 = first_parms_id, 1 = after one modulus switch, ...; k of
+        that level), or None for an empty destination."""
         R = self.ref
         h = vp()
         R.call("Ciphertext_Create1", None, C.byref(h))
         if words is not None:
             words = np.ascontiguousarray(words, dtype=np.uint64)
-            assert words.shape[1:] == (self.k, self.n), words.shape
-            rc = R.lib.refshim_ct_resize(h, self.ctx, self.first_parms_id, words.shape[0], int(ntt))
+            assert words.shape[1:] == (self.k - level, self.n), words.shape
+            pid = self.first_parms_id if level == 0 else self.data_parms_ids()[level]
+            rc = R.lib.refshim_ct_resize(h, self.ctx, pid, words.shape[0], int(ntt))
             assert rc == 0
             C.memmove(R.lib.refshim_ct_data(h), words.ctypes.data, words.nbytes)
         return h
@@ -251,6 +271,9 @@ class RefContext:
         if coeffs.size:
             C.memmove(R.lib.refshim_pt_data(h), coeffs.ctypes.data, coeffs.nbytes)
         return h
+
+    def free_pt(self, h):
+        self.ref.call("Plaintext_Destroy", h)
 
     def pt_coeffs(self, h):
         R = self.ref

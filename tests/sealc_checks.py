@@ -95,6 +95,60 @@ def evaluator_surface(S, n, moduli, t):
             assert our_code == ref_code, (hex(our_code), hex(ref_code))
 
 
+def plain_operand_parity(S, n, moduli, t):
+    """Evaluator_MultiplyPlain / AddPlain / SubPlain with the plaintext classes of parity_checks.plain_operand_classes
+    (monomials at and around the upper-half threshold, dense upper-half and >= t plaintexts, two nonzero coefficients), as
+    plaintext handles holding only their significant coefficients, then all of them at once through the
+    B200_Evaluator_PlainBatch seam: word for word against the reference, or the reference's HRESULT where it refuses."""
+    from parity_checks import plain_operand_classes
+    R = refseal.RefContext(n, moduli, t)
+    O = S.context(n, moduli, t)
+    a = refseal.appendix_b_inputs(n, moduli, t)["a"]
+    ra, oa = R.new_ct(a), O.new_ct(a)
+    classes = plain_operand_classes(n, t, np.random.default_rng(43))
+    ops = (("multiply_plain", 2), ("add_plain", 0), ("sub_plain", 1))
+    batch = {which: ([], [], []) for _, which in ops}  # plaintext handles, labels, expected words
+    opls = []
+    for label, p in classes:
+        p = p[: max(1, int(np.flatnonzero(p)[-1]) + 1)]
+        rp, op_ = R.new_pt(p), O.new_pt(p)
+        opls.append(op_)
+        for name, which in ops:
+            try:
+                rr = getattr(R, name)(ra, rp)
+            except refseal.SealError as e:
+                try:
+                    getattr(O, name)(oa, op_)
+                except SealcError as f:
+                    assert f.code == e.code, (name, label, hex(f.code), hex(e.code))
+                else:
+                    raise AssertionError(f"{name} by {label}: the reference refuses (0x{e.code:08x}), the library does not")
+                continue
+            exp = R.ct_words(rr)
+            R.free_ct(rr)
+            oo = getattr(O, name)(oa, op_)
+            eq(O.ct_words(oo), exp, f"{name} by {label}")
+            O.S.call("Ciphertext_Destroy", oo)
+            batch[which][0].append(op_)
+            batch[which][1].append(label)
+            batch[which][2].append(exp)
+        R.free_pt(rp)
+    for name, which in ops:
+        pls, labels, exps = batch[which]
+        count = len(pls)
+        dsts = [O._dst() for _ in range(count)]
+        O.S.call("B200_Evaluator_PlainBatch", O.ev, C.c_int(which), u64(count), (vp * count)(*([oa] * count)), (vp * count)(*pls),
+                 (vp * count)(*dsts))
+        for i in range(count):
+            eq(O.ct_words(dsts[i]), exps[i], f"PlainBatch {name}, item {i} ({labels[i]})")
+        for h in dsts:
+            O.S.call("Ciphertext_Destroy", h)
+    for h in opls:
+        O.S.call("Plaintext_Destroy", h)
+    R.free_ct(ra)
+    O.S.call("Ciphertext_Destroy", oa)
+
+
 def error_codes(S, R_lib, n, moduli, t):
     """HRESULT parity with the reference on the failure paths Rust maps (seal_fhe/src/error.rs:65-91)."""
     R = refseal.RefContext(n, moduli, t)
@@ -671,6 +725,53 @@ def leftovers_parity(S, n, moduli, t):
         RL.call("Decryptor_InvariantNoise", rdec, h, C.byref(a))
         OL.call("Decryptor_InvariantNoise", odec, oh, C.byref(b))
         assert a.value == b.value and 0.0 < a.value < 0.5, (a.value, b.value)
+
+
+def noise_edge_parity(S, n, moduli, t, seed=47):
+    """Decryptor_InvariantNoiseBudget and Decryptor_InvariantNoise (the Sunscreen fork's double) against the reference, values
+    and HRESULTs, on ciphertexts whose noise sits at the edges of the layer-2 host code (bit count, the max(0, .) clamp,
+    the word-by-word double): c1 = 0 and c0 = X with t X = Y (mod Q) for Y = 0 everywhere (norm 0), (Q -+ 1)/2 (norm just
+    below Q/2: budget 0), Q - 1, 2^64 - 1 and 2^64 (a word carry), at coefficients 0, 127, 128 and n - 1 over values below
+    2^20; plus random ciphertexts of size 2 and 3, whose noise is near Q/2."""
+    from parity_checks import _residues, rand_ct
+    R = refseal.RefContext(n, moduli, t)
+    O = S.context(n, moduli, t)
+    RL, OL = _libs(R, O)
+    rng = np.random.default_rng(seed)
+    kg = R.keygen()
+    sk = R.secret_key(kg)
+    rdec, odec = R.decryptor(sk), vp()
+    osk = OL.load("SecretKey", RL.save("SecretKey", sk, 0))
+    O.S.call("Decryptor_Create", O.ctx, osk, C.byref(odec))
+    q = R.data_moduli
+    Q = math.prod(q)
+    tinv = pow(t, -1, Q)
+    cases = [("norm 0", np.zeros((2, R.k, n), dtype=np.uint64))]
+    edges = [y for y in ((Q - 1) // 2, (Q + 1) // 2, Q - 1, 2**64 - 1, 2**64) if 0 < y < Q]
+    for p, pos in enumerate((0, 127, 128, n - 1)):
+        for e in range(len(edges)):
+            Y = [int(v) for v in rng.integers(0, 2**20, size=n)] if (p + e) % 2 else [0] * n
+            Y[pos] = edges[(p + e) % len(edges)]
+            ct = np.zeros((2, R.k, n), dtype=np.uint64)
+            ct[0], _ = _residues([y * tinv % Q for y in Y], q, n, rng)
+            cases.append((f"Y = {Y[pos]:#x} at {pos}", ct))
+    for size in (2, 3):
+        cases.append((f"random size {size}", rand_ct(rng, q, R.k, n, size=size)))
+    budgets = set()
+    for label, ct in cases:
+        rh, oh = R.new_ct(ct), O.new_ct(ct)
+        rb, ob, rn, on = C.c_int(-7), C.c_int(-7), C.c_double(-7.0), C.c_double(-7.0)
+        r_rc = RL.rc("Decryptor_InvariantNoiseBudget", rdec, rh, C.byref(rb))
+        o_rc = OL.rc("Decryptor_InvariantNoiseBudget", odec, oh, C.byref(ob))
+        assert (r_rc, rb.value) == (o_rc, ob.value), f"InvariantNoiseBudget, {label}: reference {r_rc:#x} {rb.value}, ours {o_rc:#x} {ob.value}"
+        r_rc = RL.rc("Decryptor_InvariantNoise", rdec, rh, C.byref(rn))
+        o_rc = OL.rc("Decryptor_InvariantNoise", odec, oh, C.byref(on))
+        assert (r_rc, rn.value) == (o_rc, on.value), f"InvariantNoise, {label}: reference {r_rc:#x} {rn.value!r}, ours {o_rc:#x} {on.value!r}"
+        budgets.add(rb.value)
+        R.free_ct(rh)
+        O.S.call("Ciphertext_Destroy", oh)
+    # the inputs reach norm 0 (the largest budget, bits(Q) - 1) and the clamp at 0
+    assert {0, Q.bit_length() - 1} <= budgets, budgets
 
 
 def _siphash13(data):

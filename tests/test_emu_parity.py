@@ -8,12 +8,12 @@ import pytest
 
 import parity_checks as pc
 from backends import EmuBackend
-from params import EDGE, PARAMS
+from params import EDGE, PARAMS, PLAIN_EDGE
 
 GOLD = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "appendix_b.json")))
 
 
-@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49"] + EDGE)
+@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49"] + EDGE + [p for p in PLAIN_EDGE if PARAMS[p][0] <= 8192])
 def pair(request, emu_lib, ref):
     return pc.pair_for(EmuBackend(emu_lib), request.param)
 
@@ -46,6 +46,12 @@ def test_galois(pair):
 
 def test_plain_ops(pair):
     pc.check_plain(pair)
+
+
+def test_plain_operands(pair):
+    if pair.n > 8192:
+        pytest.skip("plain operand classes run on n <= 8192 only (emulation speed)")
+    pc.check_plain_operands(pair)
 
 
 def test_mod_switch(pair):
@@ -82,6 +88,18 @@ def test_noise_norm(pair):
     pc.check_noise_norm(pair)
 
 
+def test_noise_norm_edges(pair):
+    if pair.n > 8192:
+        pytest.skip("noise norm edges run on n <= 8192 only (emulation speed)")
+    pc.check_noise_norm_edges(pair)
+
+
+def test_decrypt(pair):
+    if pair.n > 8192:
+        pytest.skip("decryption checks run on n <= 8192 only (emulation speed)")
+    pc.check_decrypt(pair)
+
+
 def test_encrypted_roundtrip(pair):
     pc.check_encrypted_roundtrip(pair)
 
@@ -97,6 +115,27 @@ def test_n32768_two_level_transform(emu_lib, ref):
     pc.check_galois(P)
     pc.check_plain(P)
     pc.check_modswitch(P)
+
+
+def test_wide_plain_modulus_auxiliary_base(emu_lib):
+    """n16384_t60: with a 60-bit t, the FP64 auxiliary base (49-bit primes) clears the range condition
+    32 + bits(t) + bits(Q) < bits(prod(B) * m_sk) by less than one prime's width at every level, so a count rule one prime
+    short would fail check_context there; with t = 786433 the same base has 47 to 49 bits to spare."""
+    import math
+    from sunscreen_b200.lib import B200Context
+
+    def spare_bits(name):
+        n, moduli, t = PARAMS[name]
+        ctx = B200Context(n, moduli, t, lib=emu_lib)
+        out = []
+        for lv in range(ctx.levels):
+            li = ctx.level_info(lv)
+            assert max(b.bit_length() for b in li["bsk"]) == 49
+            out.append(math.prod(li["bsk"]).bit_length() - (32 + t.bit_length() + math.prod(li["q"]).bit_length()))
+        return out
+
+    assert all(0 < s < 48 for s in spare_bits("n16384_t60")), spare_bits("n16384_t60")
+    assert all(s >= 47 for s in spare_bits("n16384")), spare_bits("n16384")
 
 
 def test_layer1_argument_checks(emu_lib):

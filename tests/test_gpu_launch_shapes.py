@@ -257,3 +257,43 @@ def test_process_wide_setting(ref, setting):
     r = subprocess.run(cmd, env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, f"{setting}: exit {r.returncode}\n{r.stdout[-2000:]}\n{r.stderr[-4000:]}"
     assert r.stdout.split() == ["ok", "n4096", "ok", "n8192", "ok", "n16384"], r.stdout
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the plain-modulus NTT (BatchEncoder) on either side of the FP64 width limit
+# ---------------------------------------------------------------------------------------------------------------------
+_PLAIN_NTT_TRACE = """
+import ctypes as C, sys
+sys.path[:0] = [{root!r}, {tests!r}]
+import numpy as np
+from backends import CudaBackend
+from sunscreen_b200.lib import B200Context, ptr
+be = CudaBackend()
+ctx = B200Context({n}, {moduli!r}, {t})
+x = be.to_dev(np.arange(4 * {n}, dtype=np.uint64) % {t})
+for inverse in (1, 0):
+    assert ctx.L.lib.b200_plain_ntt(ctx.h, C.c_void_p(ptr(x)), C.c_uint64(4), C.c_int(inverse), None) == 0
+assert np.array_equal(be.to_host(x).reshape(-1), np.arange(4 * {n}, dtype=np.uint64) % {t})
+ctx.L.lib.b200_trace_dump()
+"""
+
+
+@pytest.mark.parametrize("bits", [49, 50])
+def test_plain_ntt_fp64_width_limit(bits):
+    """n8192_t49's plain modulus is the widest the FP64 transform takes (host_ctx.h FP_PRIME_BITS = 49): with the launch
+    trace on, its BatchEncoder transforms run ntt_fp_kernel, and those of the 50-bit batching prime run the integer kernel."""
+    from test_params import batching_plain_modulus
+    from params import PARAMS
+    n, moduli, t = PARAMS["n8192_t49"]
+    if bits == 50:
+        t = batching_plain_modulus(n, 50, skip=moduli)
+    assert t.bit_length() == bits
+    env = dict(os.environ, B200_TRACE="1")
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + \
+        ["-c", _PLAIN_NTT_TRACE.format(root=ROOT, tests=HERE, n=n, moduli=moduli, t=t)]
+    r = subprocess.run(cmd, env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, f"exit {r.returncode}\n{r.stdout[-2000:]}\n{r.stderr[-4000:]}"
+    names = [m.group(1) for m in re.finditer(r"\[b200 trace\] (.+?)\s+launches\s+\d+", r.stderr)]
+    fp = [nm for nm in names if nm.startswith("ntt_fp_kernel")]
+    assert (len(fp) == 2) == (bits == 49) and (not fp) == (bits == 50), names
+    assert ("kfn" in names) == (bits == 50), names

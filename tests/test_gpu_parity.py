@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import parity_checks as pc
-from params import EDGE, PARAMS
+from params import EDGE, PARAMS, PLAIN_EDGE
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -20,7 +20,7 @@ def be():
     return CudaBackend()
 
 
-@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49", "n16384", "n32768"] + EDGE)
+@pytest.fixture(scope="module", params=["n4096", "n8192", "n8192_54", "n8192_49", "n16384", "n32768"] + EDGE + PLAIN_EDGE)
 def pair(request, be, ref):
     return pc.pair_for(be, request.param)
 
@@ -61,6 +61,10 @@ def test_plain_ops(pair):
     pc.check_plain(pair)
 
 
+def test_plain_operands(pair):
+    pc.check_plain_operands(pair)
+
+
 def test_mod_switch(pair):
     pc.check_modswitch(pair)
 
@@ -79,6 +83,14 @@ def test_small_kernels(pair):
 
 def test_noise_norm(pair):
     pc.check_noise_norm(pair)
+
+
+def test_noise_norm_edges(pair):
+    pc.check_noise_norm_edges(pair)
+
+
+def test_decrypt(pair):
+    pc.check_decrypt(pair)
 
 
 def test_encrypted_roundtrip(pair):

@@ -2,10 +2,11 @@
 CoeffModulus::Create(n, bits) returns (the reference's prime search, restated here; compared with the reference library
 itself where it is built)."""
 import ctypes as C
+import math
 
 import pytest
 
-from params import EDGE, EDGE_BITS, PARAMS, SEC_NONE
+from params import EDGE, EDGE_BITS, PARAMS, PLAIN_EDGE, PLAIN_EDGE_T, SEC_NONE
 
 
 def is_prime(v):
@@ -82,6 +83,66 @@ def test_edge_chains_reach_their_cases():
     for name, logn in (("n2048_2x27", 11), ("n1024_2x27", 10)):
         n, m, t = PARAMS[name]
         assert n == 1 << logn and len(m) == 2 and t % (2 * n) == 1
+
+
+def batching_plain_modulus(n, bits, skip=()):
+    """PlainModulus::Batching(n, bits) = CoeffModulus::Create(n, {bits})[0], the largest prime = 1 mod 2n below 2^bits;
+    with `skip`, the largest such prime not in it."""
+    return max(p for p in create_coeff_modulus(n, [bits] * (len(skip) + 1)) if p not in skip)
+
+
+@pytest.mark.parametrize("name", PLAIN_EDGE)
+def test_plain_edge_modulus(name):
+    base, rule = PLAIN_EDGE_T[name]
+    n, moduli, t = PARAMS[name]
+    assert (n, moduli) == PARAMS[base][:2]
+    if isinstance(rule, tuple):
+        assert rule[0] == "batching" and t.bit_length() == rule[1]
+        assert t == batching_plain_modulus(n, rule[1], skip=moduli)
+        assert is_prime(t) and t % (2 * n) == 1
+    else:
+        assert t == rule
+
+
+def test_plain_edge_sets_reach_their_cases():
+    """What each wide plain modulus is there for."""
+    bits = lambda q: math.prod(q).bit_length()
+    n, m, t = PARAMS["n8192_t47"]
+    assert t == batching_plain_modulus(n, 47)      # the first candidate of the 47-bit FP64 auxiliary base
+    assert max(q.bit_length() for q in m) < 47
+    n, m, t = PARAMS["n8192_60_t60"]
+    assert batching_plain_modulus(n, 60) in m and t not in m and all(q > t for q in m)
+    n, m, t = PARAMS["n8192_54_t60"]
+    k = len(m) - 1                                  # first data level: the reference's rule adds a B prime
+    assert 32 + t.bit_length() + bits(m[:k]) >= 61 * k + 61
+    assert PARAMS["n8192_t3p37"][2] % 2 == 1 and not is_prime(PARAMS["n8192_t3p37"][2])
+    # the widest plain modulus the FP64 transform takes (host_ctx.h FP_PRIME_BITS; the kernel choice itself is asserted by
+    # test_gpu_launch_shapes.py::test_plain_ntt_fp64_width_limit)
+    assert PARAMS["n8192_t49"][2].bit_length() == 49
+    # a 60-bit t on a chain whose primes all take the FP64 path (the auxiliary base's range margin is asserted by
+    # test_emu_parity.py::test_wide_plain_modulus_auxiliary_base)
+    n, m, t = PARAMS["n16384_t60"]
+    assert t.bit_length() == 60 and max(q.bit_length() for q in m) == 49
+
+
+@pytest.mark.parametrize("name", PLAIN_EDGE)
+def test_plain_edge_matches_reference(ref, name):
+    """The reference's own prime search gives the same batching t, and it accepts the set at 128-bit security."""
+    import refseal
+    base, rule = PLAIN_EDGE_T[name]
+    n, moduli, t = PARAMS[name]
+    if isinstance(rule, tuple):
+        count = len(moduli) + 1
+        arr = (C.c_int * count)(*([rule[1]] * count))
+        out = (C.c_void_p * count)()
+        ref.call("CoeffModulus_Create1", C.c_uint64(n), C.c_uint64(count), arr, out)
+        got = []
+        for h in out:
+            v = C.c_uint64()
+            ref.call("Modulus_Value", C.c_void_p(h), C.byref(v))
+            got.append(v.value)
+        assert t == max(p for p in got if p not in moduli)
+    refseal.RefContext(n, moduli, t)
 
 
 @pytest.mark.parametrize("name", EDGE)

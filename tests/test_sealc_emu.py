@@ -3,7 +3,7 @@ against our library and the reference, every word / HRESULT compared."""
 import pytest
 
 import sealc_checks as sc
-from params import PARAMS
+from params import PARAMS, PLAIN_EDGE
 from sealc_driver import Sealc
 
 
@@ -39,7 +39,7 @@ def test_chi_sq_dag_small(S, ref):
     sc.chi_sq_dag(S, *PARAMS["n8192"], evaluations=1)
 
 
-@pytest.mark.parametrize("name", ["n8192"])
+@pytest.mark.parametrize("name", ["n8192"] + [p for p in PLAIN_EDGE if PARAMS[p][0] <= 8192 and PARAMS[p][2] % (2 * PARAMS[p][0]) == 1])
 def test_batch_encoder(S, ref, name):
     sc.batch_encoder_parity(S, *PARAMS[name])
 
@@ -72,9 +72,19 @@ def test_single_prime_chain(S, ref, n, moduli, t):
     sc.single_prime_context(S, n, moduli, t)
 
 
-@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_sealfhe", "n4096_q_below_t"])
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_sealfhe", "n4096_q_below_t"] + [p for p in PLAIN_EDGE if PARAMS[p][0] <= 8192])
 def test_whole_chain_and_large_sizes(S, ref, name):
     sc.deep_chain_parity(S, *PARAMS[name])
+
+
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n4096_q_below_t", "n4096_t2", "n8192_60_t60"])
+def test_plain_operand_classes(S, ref, name):
+    sc.plain_operand_parity(S, *PARAMS[name])
+
+
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n4096_t2p40"])
+def test_noise_budget_edges(S, ref, name):
+    sc.noise_edge_parity(S, *PARAMS[name])
 
 
 @pytest.mark.parametrize("name", ["n4096", "n8192"])

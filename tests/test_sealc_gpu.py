@@ -5,7 +5,7 @@ import os
 import pytest
 
 import sealc_checks as sc
-from params import PARAMS
+from params import PARAMS, PLAIN_EDGE
 from sealc_driver import Sealc
 
 pytestmark = pytest.mark.gpu
@@ -112,7 +112,7 @@ def test_config5_rotate_multiply_plain_sweep_n32768(S, ref):
     sc.rotate_multiply_plain_sweep(S, *PARAMS["n32768"], steps=(1, 2, 4, 64, 1024, 8192))
 
 
-@pytest.mark.parametrize("name", ["n8192", "n16384", "n32768"])
+@pytest.mark.parametrize("name", ["n8192", "n16384", "n32768"] + [p for p in PLAIN_EDGE if PARAMS[p][2] % (2 * PARAMS[p][0]) == 1])
 def test_batch_encoder(S, ref, name):
     sc.batch_encoder_parity(S, *PARAMS[name])
 
@@ -145,9 +145,19 @@ def test_single_prime_chain(S, ref, n, moduli, t):
     sc.single_prime_context(S, n, moduli, t)
 
 
-@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_49", "n16384", "n8192_sealfhe", "n16384_mixed"])
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n8192_49", "n16384", "n8192_sealfhe", "n16384_mixed"] + PLAIN_EDGE)
 def test_whole_chain_and_large_sizes(S, ref, name):
     sc.deep_chain_parity(S, *PARAMS[name])
+
+
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n16384", "n32768", "n4096_q_below_t", "n4096_t2", "n8192_60_t60", "n16384_t60"])
+def test_plain_operand_classes(S, ref, name):
+    sc.plain_operand_parity(S, *PARAMS[name])
+
+
+@pytest.mark.parametrize("name", ["n4096", "n8192", "n16384", "n32768", "n8192_60_t60"])
+def test_noise_budget_edges(S, ref, name):
+    sc.noise_edge_parity(S, *PARAMS[name])
 
 
 @pytest.mark.parametrize("name", ["n4096", "n8192"])
