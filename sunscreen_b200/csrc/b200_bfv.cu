@@ -125,6 +125,7 @@ __global__ void __launch_bounds__(NT, MB) ntt_kernel(const NttJob job)
 #ifndef B200_EMU_HEADER
 #include "ntt_fp_kernels.h"
 #include "ksmac_tma.h"
+#include "mul_cluster.h"
 #endif
 
 #define GLOBAL_IDX() ((long long)blockIdx.x * blockDim.x + threadIdx.x)
@@ -828,6 +829,7 @@ struct b200_ctx
     std::unique_ptr<BfvHostContext> host;
     int device = 0;
     int sm_count = 0;
+    int mul_clusters = 0; // 4-CTA clusters of mul_cluster_kernel the device holds at once (0: no cluster kernel for this size)
     size_t n = 0;
     int logn = 0;
     std::vector<void *> allocations; // everything freed at destroy
@@ -1609,6 +1611,7 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
         return rc;
     if ((rc = scr.get((size_t)batch * Dn * R * n, &D)))
         return rc;
+    bool clustered = false; // (3)-(5) ran as mul_cluster_kernel
     // (1)-(2) lift to Bsk
     {
         if (L.fp)
@@ -1625,7 +1628,53 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
         }
         ctx->launches++;
     }
+#ifndef B200_EMU_HEADER
+    // (3)-(5) in one kernel for a size-2 x size-2 product on the FP64 static path (mul_cluster.cu): the NTT-form operands and
+    // products stay in the shared memory of a 4-CTA cluster.  Taken where the launch fills the GPU (the rule of the 256/512
+    // thread switch in launch_ntt); B200_MUL_CLUSTER=0 selects the separate kernels below, B200_TENSOR_FUSION=1 their fused
+    // inverse copy-in.
+    static const bool want_cluster = !(std::getenv("B200_MUL_CLUSTER") && std::getenv("B200_MUL_CLUSTER")[0] == '0') &&
+                                     !std::getenv("B200_TENSOR_FUSION");
+    if (want_cluster && !square && sa == 2 && sb == 2 && L.fp && ctx->mul_clusters > 0 && ctx->logn <= 13 &&
+        4LL * R * batch > 2LL * ctx->sm_count)
+    {
+        JobDesc jd;
+        if ((rc = get_job(ctx, "mulcl:" + std::to_string(level), row_primes(ctx, level, true), {}, {}, &jd)))
+            return rc;
+        if (static_fp_ok(ctx, jd))
+        {
+            if (4LL * R * batch > 0x7fffffffLL)
+                return fail(B200_E_INVALID, "batch too large for one multiply launch");
+            NttJob job;
+            memset(&job, 0, sizeof(job));
+            job.logn = ctx->logn;
+            job.slots = R;
+            job.slot_prime = jd.d_prime;
+            job.primes = ctx->d_ntt_primes;
+            job.fprimes = ctx->d_fp_primes;
+            job.items = batch;
+            cudaEvent_t t0 = nullptr, t1 = nullptr;
+            if (trace_on())
+            {
+                cudaEventCreate(&t0);
+                cudaEventCreate(&t1);
+                cudaEventRecord(t0, s);
+            }
+            const int crc = b200_mul_cluster(ctx->logn, job, a, b, ext, D, k, s);
+            if (crc)
+                return fail(B200_E_CUDA, std::string("mul_cluster_kernel: ") + cudaGetErrorString((cudaError_t)crc));
+            if (t0)
+            {
+                cudaEventRecord(t1, s);
+                g_trace.push_back(B200TraceRec{ "mul_cluster_kernel", t0, t1 });
+            }
+            ctx->launches++;
+            clustered = true;
+        }
+    }
+#endif
     // (3) forward NTTs in ONE launch: q rows straight from the inputs (alternative sources a, b), Bsk rows in place in ext
+    if (!clustered)
     {
         std::vector<int> prime;
         std::vector<long long> so, dof;
@@ -1663,6 +1712,7 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
     }
     // (4) tensor + (5) inverse NTTs.  Optionally (FP64 path) the dyadic products are formed inside the inverse
     // transform's coalesced copy-in (D never materialised in NTT form); by default a separate tensor kernel runs.
+    if (!clustered)
     {
         std::vector<int> rows = row_primes(ctx, level, true), prime;
         for (int m = 0; m < Dn; m++)
@@ -1900,6 +1950,9 @@ int b200_ctx_create(uint64_t n, const uint64_t *coeff_modulus, uint64_t count, u
         const int frc = b200_ntt_fp_setup((int)prop.sharedMemPerBlockOptin);
         if (frc)
             return fail(B200_E_CUDA, std::string("cudaFuncSetAttribute (FP64 NTT kernels): ") + cudaGetErrorString((cudaError_t)frc));
+        const int crc = b200_mul_cluster_setup(ctx->logn, &ctx->mul_clusters);
+        if (crc)
+            return fail(B200_E_CUDA, std::string("mul_cluster_kernel setup: ") + cudaGetErrorString((cudaError_t)crc));
     }
 #endif
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));

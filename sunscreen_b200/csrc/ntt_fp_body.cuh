@@ -518,7 +518,11 @@ struct NttFpStaticPass
             else
                 asm volatile("bar.sync %0, %1;" ::"r"(1 + wwarp), "r"(WP_TG) : "memory");
         };
-        constexpr bool SG = EDGE_IN && LOGS >= 5 && B200_NTT_DIRECT_IN && !STREAM, DG = EDGE_OUT && LOGS >= 5 && !(VAR & 128); // 128: always stage the output
+        // VAR & 4096: the polynomial stays in shared memory at the hand-off to / from the fused dyadic step (mul_cluster.cu): the
+        // forward transform leaves its lazy result there (no copy-out), the inverse finds canonical values there (no copy-in)
+        constexpr bool KEEP_OUT = (VAR & 4096) != 0 && FWD, SMEM_IN = (VAR & 4096) != 0 && !FWD;
+        constexpr bool SG = EDGE_IN && LOGS >= 5 && B200_NTT_DIRECT_IN && !STREAM && !SMEM_IN,
+                       DG = EDGE_OUT && LOGS >= 5 && !(VAR & 128) && !KEEP_OUT; // 128: always stage the output
         constexpr bool TW16 = (L == 4 && LOGS == 0);
         constexpr int TWSRC = (VAR & 2) ? 2 : ((VAR & 1) && !TW16 && (1 << (DONE + L)) <= B200_NTT_TWS_ENTRIES) ? 1 : 0;
         constexpr int ABL = ((VAR & 4) ? 1 : 0) | ((VAR & (8 | 32)) ? 2 : 0) | ((VAR & (8 | 64)) ? 4 : 0) | ((VAR & 512) ? 8 : 0); // 32 / 64: loads / stores only; 512: streaming (evict-first) hints
@@ -537,7 +541,9 @@ struct NttFpStaticPass
         const bool red = EDGE_IN && job.reduce_input != 0;
         const int ptid = ntt_pad(tid);              // NT is a multiple of 16: pad(tid + it*NT) = pad(tid) + it*(NT + NT/16)
         constexpr int PNT = NT + (NT >> 4);
-        if (EDGE_IN && !SG)
+        if constexpr (EDGE_IN && SMEM_IN)
+            __syncthreads(); // the whole CTA's twiddle copy above is complete (the first pass may span other warps' values)
+        else if (EDGE_IN && !SG)
         { // coalesced copy-in: u64 -> double
             if (!FWD && job.tensor_mode)
             {
@@ -625,7 +631,7 @@ struct NttFpStaticPass
                 job.timeline[(unsigned long long)blockIdx.x * 8 + 6] = t; // copy-in complete
             }
         }
-        constexpr bool RAW = EDGE_IN && !SG; // (the tensor-fused copy-in writes doubles: handled by the run-time flag below)
+        constexpr bool RAW = EDGE_IN && !SG && !SMEM_IN; // (the tensor-fused copy-in writes doubles: handled by the run-time flag below)
         // renormalisation / input reduction are block-uniform run-time flags: branch ONCE to a compile-time variant
         // (as predicated code they cost 12 FP64 ops and ~10 IMADs per element whether needed or not)
         // group handled by this thread in iteration `it`: block-strided by default, inside the warp's own block when warp-private
@@ -793,7 +799,7 @@ struct NttFpStaticPass
             asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
             job.timeline[(unsigned long long)blockIdx.x * 8 + 2 + STEP] = t;
         }
-        if (EDGE_OUT && !DG && !(STREAM && FWD))
+        if (EDGE_OUT && !DG && !(STREAM && FWD) && !KEEP_OUT)
         { // coalesced copy-out: lazy double -> canonical u64
             if constexpr ((VAR & 256) != 0)
             { // two adjacent words per thread: one 128-bit store (the pair never straddles a pad: even index, runs of 16)

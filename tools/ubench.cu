@@ -309,6 +309,85 @@ __global__ void k_bf_mixed(u64 *out, const u64 *tw, u64 p)
     }
 }
 
+// ---- distributed shared memory (DSMEM) across a 4-CTA cluster: the hand-off of mul_cluster.cu ----
+// Every CTA holds one padded n = 8192 polynomial (the NTT kernels' shared-memory footprint, 3 CTAs/SM); each pass every thread
+// touches its 32 words once, in the CTA `pass % 3 + 1` ranks ahead (MODE 0: local ld.shared, 1: remote ld.shared::cluster,
+// 2: remote st.shared::cluster).
+#define DS_N 8192
+#define DS_WORDS (DS_N + DS_N / 16)
+template <int MODE>
+__global__ void __launch_bounds__(256, 3) k_dsmem(double *out, int passes)
+{
+    extern __shared__ double ds[];
+    unsigned rank;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
+    for (int e = threadIdx.x; e < DS_WORDS; e += 256)
+        ds[e] = e + rank;
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+    double acc = 0.0;
+    for (int ps = 0; ps < passes; ps++)
+    {
+        const unsigned peer = MODE == 0 ? rank : (rank + 1 + ps % 3) & 3;
+#pragma unroll 8
+        for (int it = 0; it < DS_N / 256; it++)
+        {
+            const int e = threadIdx.x + it * 256;
+            const unsigned la = (unsigned)__cvta_generic_to_shared(ds + e + (e >> 4));
+            unsigned ra;
+            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(la), "r"(peer));
+            if (MODE == 2)
+                asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(ra), "d"(acc + e) : "memory");
+            else
+            {
+                double v;
+                asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(ra) : "memory");
+                acc += v;
+            }
+        }
+    }
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+    out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
+}
+
+template <int MODE>
+static float dsmem_run(double *out, int clusters, int passes)
+{
+    const size_t smem = DS_WORDS * sizeof(double);
+    cudaFuncSetAttribute(k_dsmem<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = 4;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3(4 * clusters);
+    cfg.blockDim = dim3(256);
+    cfg.dynamicSmemBytes = smem;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    if (MODE == 0)
+    {
+        int active = 0;
+        cudaOccupancyMaxActiveClusters(&active, k_dsmem<MODE>, &cfg);
+        printf("dsmem: %d active 4-CTA clusters (%d CTAs), %zu B shared memory per CTA\n", active, 4 * active, smem);
+    }
+    cudaEvent_t a, b;
+    cudaEventCreate(&a);
+    cudaEventCreate(&b);
+    cudaLaunchKernelEx(&cfg, k_dsmem<MODE>, out, passes);
+    cudaDeviceSynchronize();
+    cudaEventRecord(a);
+    cudaLaunchKernelEx(&cfg, k_dsmem<MODE>, out, passes);
+    cudaEventRecord(b);
+    cudaEventSynchronize(b);
+    float ms = 0;
+    cudaEventElapsedTime(&ms, a, b);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess)
+        printf("dsmem: %s\n", cudaGetErrorString(e));
+    return ms;
+}
+
 template <class F>
 float timeit(F f)
 {
@@ -383,6 +462,20 @@ int main()
         double bfs = (double)blocks * threads * (ITERS / 8) * 12;
         printf("%-20s %8.3f ms  %8.2f G butterflies/s -> %.2f M NTT(8192)/s\n", "bf mixed int+fp64", ms, bfs / ms / 1e6,
                bfs / ms / 1e3 / 53248.0);
+    }
+    {
+        // 3 CTAs per SM, whole clusters: 99 clusters on 132 SMs
+        const int clusters = sms * 3 / 4, passes = 256;
+        double *dout;
+        cudaMalloc(&dout, (size_t)clusters * 4 * 256 * sizeof(double));
+        const char *dn[] = { "dsmem local ld", "dsmem remote ld", "dsmem remote st" };
+        float ms[3] = { dsmem_run<0>(dout, clusters, passes), dsmem_run<1>(dout, clusters, passes), dsmem_run<2>(dout, clusters, passes) };
+        for (int m = 0; m < 3; m++)
+        {
+            const double bytes = (double)clusters * 4 * passes * DS_N * sizeof(double);
+            printf("%-20s %8.3f ms  %8.2f TB/s aggregate\n", dn[m], ms[m], bytes / ms[m] / 1e9);
+        }
+        cudaFree(dout);
     }
     return 0;
 }
