@@ -830,6 +830,7 @@ struct b200_ctx
     int device = 0;
     int sm_count = 0;
     int mul_clusters = 0; // 4-CTA clusters of mul_cluster_kernel the device holds at once (0: no cluster kernel for this size)
+    int ks_clusters[9] = {}; // [k]: k-CTA clusters of ks_cluster_kernel the device holds at once (0: no cluster kernel)
     size_t n = 0;
     int logn = 0;
     std::vector<void *> allocations; // everything freed at destroy
@@ -1786,10 +1787,59 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
     Scratch scr(ctx, s);
     u64 *ks1 = nullptr, *ks2 = nullptr;
     int rc;
-    if ((rc = scr.get((size_t)batch * (k + 1) * k * n, &ks1)))
-        return rc;
     if ((rc = scr.get((size_t)batch * 2 * (k + 1) * n, &ks2)))
         return rc;
+    bool clustered = false; // the forward NTTs, the inner product and the inverse NTTs ran as ks_cluster_kernel
+#ifndef B200_EMU_HEADER
+    // all three in one kernel on the FP64 static path (mul_cluster.cu): the transformed digits and the accumulators stay in the
+    // shared memory of a k-CTA cluster.  Taken where the launch fills the GPU (the rule of the 256/512 thread switch in
+    // launch_ntt and of the multiply's cluster); B200_KS_CLUSTER=0 selects the separate kernels below.
+    static const bool want_cluster = !(std::getenv("B200_KS_CLUSTER") && std::getenv("B200_KS_CLUSTER")[0] == '0');
+    if (want_cluster && L.fp && ctx->logn <= 13 && k >= 2 && k <= 8 && ctx->ks_clusters[k] > 0 &&
+        (long long)k * (k + 1) * batch > 2LL * ctx->sm_count)
+    {
+        std::vector<int> prime;
+        for (int I = 0; I <= k; I++)
+            prime.push_back(I < k ? Lh.q_idx[I] : special);
+        JobDesc jd;
+        if ((rc = get_job(ctx, "kscl:" + std::to_string(level), prime, {}, {}, &jd)))
+            return rc;
+        if (static_fp_ok(ctx, jd))
+        {
+            if ((long long)k * (k + 1) * batch > 0x7fffffffLL)
+                return fail(B200_E_INVALID, "batch too large for one key-switch launch");
+            NttJob job;
+            memset(&job, 0, sizeof(job));
+            job.logn = ctx->logn;
+            job.slots = k + 1;
+            job.slot_prime = jd.d_prime;
+            job.primes = ctx->d_ntt_primes;
+            job.fprimes = ctx->d_fp_primes;
+            job.reduce_input = 1;
+            job.items = batch;
+            cudaEvent_t t0 = nullptr, t1 = nullptr;
+            if (trace_on())
+            {
+                cudaEventCreate(&t0);
+                cudaEventCreate(&t1);
+                cudaEventRecord(t0, s);
+            }
+            const int crc = b200_ks_cluster(ctx->logn, job, d, d_stride, key, Kkey, ks2, k, s);
+            if (crc)
+                return fail(B200_E_CUDA, std::string("ks_cluster_kernel: ") + cudaGetErrorString((cudaError_t)crc));
+            if (t0)
+            {
+                cudaEventRecord(t1, s);
+                g_trace.push_back(B200TraceRec{ "ks_cluster_kernel", t0, t1 });
+            }
+            ctx->launches++;
+            clustered = true;
+        }
+    }
+#endif
+    if (!clustered && (rc = scr.get((size_t)batch * (k + 1) * k * n, &ks1)))
+        return rc;
+    if (!clustered)
     {
         std::vector<int> prime;
         std::vector<long long> so, dof;
@@ -1806,6 +1856,7 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         if ((rc = launch_ntt<true>(ctx, jd, d, d_stride, ks1, (long long)(k + 1) * k * n, batch, 1, s)))
             return rc;
     }
+    if (!clustered)
     {
         bool done = false;
 #ifndef B200_EMU_HEADER
@@ -1855,6 +1906,7 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         }
         ctx->launches++;
     }
+    if (!clustered)
     {
         std::vector<int> prime;
         for (int comp = 0; comp < 2; comp++)
@@ -1953,6 +2005,12 @@ int b200_ctx_create(uint64_t n, const uint64_t *coeff_modulus, uint64_t count, u
         const int crc = b200_mul_cluster_setup(ctx->logn, &ctx->mul_clusters);
         if (crc)
             return fail(B200_E_CUDA, std::string("mul_cluster_kernel setup: ") + cudaGetErrorString((cudaError_t)crc));
+        for (int k = 2; k <= 8; k++)
+        {
+            const int krc = b200_ks_cluster_setup(ctx->logn, k, &ctx->ks_clusters[k]);
+            if (krc)
+                return fail(B200_E_CUDA, std::string("ks_cluster_kernel setup: ") + cudaGetErrorString((cudaError_t)krc));
+        }
     }
 #endif
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));

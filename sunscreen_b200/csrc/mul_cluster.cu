@@ -12,6 +12,11 @@
 // words the forward transform would have written), the products are formed by the arithmetic of tensor_coeff_fp
 // (bfv_body.cuh) and brought to canonical form again (the words the tensor kernel would have written), so the inverse
 // transform starts from the inputs, and the magnitude bounds (renorm masks), it has today.
+//
+// ks_cluster_kernel gives the key switch the same treatment: a k-CTA cluster per (item, key residue I) transforms the k digits
+// mod p_I, forms the two inner products with the key and transforms them back, instead of the ks1 NTT, the MAC and the ks2 NTT
+// of keyswitch_core.  Its hand-offs are canonical as well: the digits before the products (the words of ks1), the accumulators
+// (the words of ks2, formed by the FP64 branch of ksmac_tma_kernel), so every word and every renorm bound equals the separate path's.
 #include "mul_cluster.h"
 #include "ntt_fp_body.cuh"
 #include <cuda_runtime.h>
@@ -124,15 +129,124 @@ __global__ void __launch_bounds__(NT, 3) mul_cluster_kernel(const NttJob job, co
     NttFpStaticPass<LOGN, NT, false, 0, INV_VAR>::run(job, PFi, job.primes[job.slot_prime[w.r]], nullptr, dst, smd, tid, w.item, w.r);
 }
 
+// ks_cluster_kernel's place: rank J in the cluster (digit J), key residue I in [0, k] (k: the special prime), item.  Items
+// outermost: the k + 1 clusters of an item run together, so its k digit rows come from HBM once and from L2 the other k times
+struct KsPlace
+{
+    int J, I;
+    long long item;
+};
+__device__ __forceinline__ KsPlace ks_place(int k)
+{
+    unsigned J, blk;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(J));
+    asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(blk));
+    const unsigned cl = blk / (unsigned)k, item = cl / (unsigned)(k + 1);
+    return KsPlace{ (int)J, (int)(cl - item * (unsigned)(k + 1)), (long long)item };
+}
+
+// The key switch's NTT-domain half for one (item, key residue I): forward transforms of the k digits mod p_I, inner product
+// with the key, inverse transforms of the two accumulators into ks2 [item][2][k + 1][n] (coefficient form, canonical).
 template <int LOGN>
-cudaLaunchConfig_t config(long long clusters, cudaLaunchAttribute *at, cudaStream_t s)
+__global__ void __launch_bounds__(NT, 3) ks_cluster_kernel(const NttJob job, const u64 *d, long long d_stride, const u64 *key, int key_rows,
+                                                           u64 *ks2, int k)
+{
+    extern __shared__ u64 mc_sm[];
+    constexpr int N = 1 << LOGN;
+    double *smd = reinterpret_cast<double *>(mc_sm);
+    const int tid = (int)threadIdx.x;
+    KsPlace w = ks_place(k);
+    {
+        const NttPrimeFp PF = job.fprimes[job.slot_prime[w.I]];
+        const NttPrime PI_ = job.primes[job.slot_prime[w.I]];
+        // digit J of the target, reduced mod p_I by the first pass (job.reduce_input)
+        NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR>::run(job, PF, PI_, d + w.item * d_stride + (long long)w.J * N, nullptr, smd, tid, w.item, w.I);
+    }
+    cluster_sync(); // all k digits transformed
+    w = ks_place(k);
+
+    // inner product: CTA J owns the chunks of NT coefficients J, J + k, J + 2k, ...; each coefficient is read (k CTAs) and
+    // written (CTAs 0, 1) by one thread only, so the in-place overwrite of digits 0 and 1 by acc_0 and acc_1 has no hazard
+    {
+        const NttPrimeFp PF = job.fprimes[job.slot_prime[w.I]];
+        const double p = PF.p, pinv = PF.pinv;
+        const unsigned base = (unsigned)__cvta_generic_to_shared(smd);
+        unsigned r0, r1;
+        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r0) : "r"(base), "r"(0));
+        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r1) : "r"(base), "r"(1));
+        // key[J][c][residue][coeff]: the special prime's row is the last key residue
+        const long long kstride = (long long)key_rows * N;
+        const u64 *kr = key + (long long)(w.I < k ? w.I : key_rows - 1) * N + tid;
+        // U chunks per round: their k remote loads and 2k key loads are issued per digit together (n = 4096: two, as in
+        // mul_cluster_kernel a wider round makes ptxas spill)
+        constexpr int CH = N / NT, U = LOGN >= 13 ? 4 : 2;
+#pragma unroll 1
+        for (int ch = w.J; ch < CH; ch += U * k)
+        {
+            unsigned off[U];
+            int e[U];
+            double a0[U], a1[U];
+#pragma unroll
+            for (int u = 0; u < U; u++)
+            {
+                e[u] = (ch + u * k) * NT;
+                off[u] = (unsigned)ntt_pad(e[u] + tid) * 8u;
+                a0[u] = 0.0;
+                a1[u] = 0.0;
+            }
+#pragma unroll 1
+            for (int J = 0; J < k; J++)
+            {
+                unsigned rj;
+                asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rj) : "r"(base), "r"(J));
+                const u64 *k0 = kr + (long long)(2 * J) * kstride, *k1 = k0 + kstride;
+                double x[U];
+                u64 y0[U], y1[U];
+#pragma unroll
+                for (int u = 0; u < U; u++)
+                    if (ch + u * k < CH)
+                    {
+                        asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(x[u]) : "r"(rj + off[u]) : "memory");
+                        y0[u] = __ldg(k0 + e[u]);
+                        y1[u] = __ldg(k1 + e[u]);
+                    }
+#pragma unroll
+                for (int u = 0; u < U; u++)
+                    if (ch + u * k < CH)
+                    {
+                        // the FP64 branch of ksmac_tma_kernel, term order included, on the words the forward NTT would have written
+                        const double xc = to_canonical(x[u], p, pinv);
+                        a0[u] = B200_DADD(a0[u], fp_mulmod2(xc, fp_from_u64(y0[u]), p, pinv));
+                        a1[u] = B200_DADD(a1[u], fp_mulmod2(xc, fp_from_u64(y1[u]), p, pinv));
+                    }
+            }
+#pragma unroll
+            for (int u = 0; u < U; u++)
+                if (ch + u * k < CH)
+                {
+                    asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(r0 + off[u]), "d"(to_canonical(a0[u], p, pinv)) : "memory");
+                    asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(r1 + off[u]), "d"(to_canonical(a1[u], p, pinv)) : "memory");
+                }
+        }
+    }
+    cluster_sync(); // acc_0, acc_1 in place; nothing reads the shared memory of CTAs 2 .. k-1 after this
+    w = ks_place(k);
+    if (w.J >= 2)
+        return;
+    u64 *dst = ks2 + ((w.item * 2 + w.J) * (k + 1) + w.I) * N;
+    const int pi = job.slot_prime[w.I]; // (loaded again: nothing of the inner product stays live)
+    NttFpStaticPass<LOGN, NT, false, 0, INV_VAR>::run(job, job.fprimes[pi], job.primes[pi], nullptr, dst, smd, tid, w.item, w.I);
+}
+
+template <int LOGN>
+cudaLaunchConfig_t config(long long clusters, cudaLaunchAttribute *at, cudaStream_t s, int csize = CLUSTER)
 {
     at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = CLUSTER;
+    at[0].val.clusterDim.x = csize;
     at[0].val.clusterDim.y = 1;
     at[0].val.clusterDim.z = 1;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(clusters * CLUSTER));
+    cfg.gridDim = dim3((unsigned)(clusters * csize));
     cfg.blockDim = dim3(NT);
     cfg.dynamicSmemBytes = smem_bytes<LOGN>();
     cfg.stream = s;
@@ -141,17 +255,18 @@ cudaLaunchConfig_t config(long long clusters, cudaLaunchAttribute *at, cudaStrea
     return cfg;
 }
 
-template <int LOGN>
-int setup(int *active)
+// shared-memory attributes of a cluster kernel, and how many clusters of `csize` CTAs of it the device holds at once
+template <int LOGN, typename KERNEL>
+int setup(KERNEL kernel, int csize, int *active)
 {
     cudaError_t e;
-    if ((e = cudaFuncSetAttribute(mul_cluster_kernel<LOGN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<LOGN>())) != cudaSuccess)
+    if ((e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<LOGN>())) != cudaSuccess)
         return (int)e;
-    if ((e = cudaFuncSetAttribute(mul_cluster_kernel<LOGN>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)) != cudaSuccess)
+    if ((e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100)) != cudaSuccess)
         return (int)e;
     cudaLaunchAttribute at[1];
-    const cudaLaunchConfig_t cfg = config<LOGN>(1, at, nullptr);
-    return (int)cudaOccupancyMaxActiveClusters(active, mul_cluster_kernel<LOGN>, &cfg);
+    const cudaLaunchConfig_t cfg = config<LOGN>(1, at, nullptr, csize);
+    return (int)cudaOccupancyMaxActiveClusters(active, kernel, &cfg);
 }
 } // namespace
 
@@ -159,9 +274,9 @@ int b200_mul_cluster_setup(int logn, int *active)
 {
     *active = 0;
     if (logn == 12)
-        return setup<12>(active);
+        return setup<12>(mul_cluster_kernel<12>, CLUSTER, active);
     if (logn == 13)
-        return setup<13>(active);
+        return setup<13>(mul_cluster_kernel<13>, CLUSTER, active);
     return 0;
 }
 
@@ -178,6 +293,37 @@ int b200_mul_cluster(int logn, const NttJob &job, const u64 *a, const u64 *b, co
     {
         const cudaLaunchConfig_t cfg = config<13>(clusters, at, (cudaStream_t)stream);
         return (int)cudaLaunchKernelEx(&cfg, mul_cluster_kernel<13>, job, a, b, ext, D, k);
+    }
+    return (int)cudaErrorInvalidValue;
+}
+
+int b200_ks_cluster_setup(int logn, int k, int *active)
+{
+    *active = 0;
+    if (k < 2 || k > 8)
+        return 0;
+    if (logn == 12)
+        return setup<12>(ks_cluster_kernel<12>, k, active);
+    if (logn == 13)
+        return setup<13>(ks_cluster_kernel<13>, k, active);
+    return 0;
+}
+
+int b200_ks_cluster(int logn, const NttJob &job, const u64 *d, long long d_stride, const u64 *key, int key_rows, u64 *ks2, int k, void *stream)
+{
+    cudaLaunchAttribute at[1];
+    const long long clusters = job.items * (k + 1);
+    if (k < 2 || k > 8)
+        return (int)cudaErrorInvalidValue;
+    if (logn == 12)
+    {
+        const cudaLaunchConfig_t cfg = config<12>(clusters, at, (cudaStream_t)stream, k);
+        return (int)cudaLaunchKernelEx(&cfg, ks_cluster_kernel<12>, job, d, d_stride, key, key_rows, ks2, k);
+    }
+    if (logn == 13)
+    {
+        const cudaLaunchConfig_t cfg = config<13>(clusters, at, (cudaStream_t)stream, k);
+        return (int)cudaLaunchKernelEx(&cfg, ks_cluster_kernel<13>, job, d, d_stride, key, key_rows, ks2, k);
     }
     return (int)cudaErrorInvalidValue;
 }
