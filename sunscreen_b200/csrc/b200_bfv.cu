@@ -258,10 +258,12 @@ static inline void stg2(u64 *p, u64 a, u64 b)
     p[0] = a;
     p[1] = b;
 }
+#define B200_DEV static inline
 #else
 typedef ulonglong2 b200_u64x2;
 __device__ __forceinline__ ulonglong2 ldg2(const u64 *p) { return __ldg(reinterpret_cast<const b200_u64x2 *>(p)); }
 __device__ __forceinline__ void stg2(u64 *p, u64 a, u64 b) { *reinterpret_cast<ulonglong2 *>(p) = make_ulonglong2(a, b); }
+#define B200_DEV __device__ __forceinline__
 #endif
 
 template <int K>
@@ -334,21 +336,13 @@ __global__ void tensor_kernel_v2(const LevelDev L, const u64 *ext, u64 *D, long 
         stg2(Dp + m * ps, out[0][m], out[1][m]);
 }
 
+// BEHZ steps 6-8 of two adjacent coefficients: src = the k + |Bsk| rows of one product at coefficient c; out[u][i] = the
+// canonical residue mod q_i of coefficient c + u
 template <int K>
-__global__ void scale_kernel_v2(const ScaleFpC<K> L, const u64 *D, int Dn, u64 *dst0, int split, u64 *dst1, long long n, long long total)
+B200_DEV void scale2_fp(const ScaleFpC<K> &L, const u64 *src, long long n, u64 (&out)[2][K])
 {
-    const long long idx = GLOBAL_IDX();
-    if (idx >= total)
-        return;
     const int R = K + L.nBsk;
-    const long long hn = n >> 1;
-    const long long c = (idx % hn) * 2;
-    const long long t = idx / hn;
-    const int m = (int)(t % Dn);
-    const long long item = t / Dn;
-    const u64 *src = D + ((item * Dn + m) * R) * n + c;
-    u64 *dst = (m < split ? dst0 + ((item * split + m) * K) * n : dst1 + ((item * (Dn - split) + (m - split)) * K) * n) + c;
-    u64 in[2][2 * K + 2], out[2][K];
+    u64 in[2][2 * K + 2];
 #pragma unroll
     for (int i = 0; i < 2 * K + 2; i++)
         if (i < R)
@@ -359,6 +353,25 @@ __global__ void scale_kernel_v2(const ScaleFpC<K> L, const u64 *D, int Dn, u64 *
         }
     scale_coeff_fp<K>(L, in[0], out[0], 1, 0);
     scale_coeff_fp<K>(L, in[1], out[1], 1, 0);
+}
+
+// products [m0, Dn) of D; product m goes to dst0 if m < split, else to dst1
+template <int K>
+__global__ void scale_kernel_v2(const ScaleFpC<K> L, const u64 *D, int Dn, int m0, u64 *dst0, int split, u64 *dst1, long long n,
+                                long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const int R = K + L.nBsk;
+    const long long hn = n >> 1;
+    const long long c = (idx % hn) * 2;
+    const long long t = idx / hn;
+    const int m = m0 + (int)(t % (Dn - m0));
+    const long long item = t / (Dn - m0);
+    u64 *dst = (m < split ? dst0 + ((item * split + m) * K) * n : dst1 + ((item * (Dn - split) + (m - split)) * K) * n) + c;
+    u64 out[2][K];
+    scale2_fp<K>(L, D + ((item * Dn + m) * R) * n + c, n, out);
 #pragma unroll
     for (int i = 0; i < K; i++)
         stg2(dst + i * n, out[0][i], out[1][i]);
@@ -419,25 +432,13 @@ __global__ void ksmoddown_kernel(const PrimeDev *primes, int special_idx, const 
     ksmoddown_coeff<K>(primes, SP, inv_qsp, acc, n, base, d, c);
 }
 
-// the same, two adjacent coefficients per thread: 128-bit loads / stores (the kernel is a pure stream of 2(k+1) + k rows in,
-// 2k rows out per item)
+// the key-switch mod-down of two adjacent coefficients: acc = the k + 1 ks2 rows of one component at coefficient c;
+// d row i = moddown(acc)_i + base[.][i] (mod q_i), base canonical
 template <int K>
-__global__ void ksmoddown_kernel_v2(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *ks2,
-                                    const u64 *base0, long long base0_stride, const u64 *base1, long long base1_stride,
-                                    u64 *dst, long long dst_item_stride, long long n, long long total)
+B200_DEV void ksmoddown2(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *acc, long long n,
+                         const u64 (&base)[2][K], u64 *d)
 {
-    const long long idx = GLOBAL_IDX();
-    if (idx >= total)
-        return;
-    const long long hn = n >> 1;
-    const long long c = (idx % hn) * 2;
-    const long long t = idx / hn;
-    const int comp = (int)(t & 1);
-    const long long item = t >> 1;
     const PrimeDev SP = ld_prime(&primes[special_idx]);
-    const u64 *acc = ks2 + ((item * 2 + comp) * (K + 1)) * n + c;
-    const u64 *base = comp == 0 ? (base0 ? base0 + item * base0_stride : nullptr) : (base1 ? base1 + item * base1_stride : nullptr);
-    u64 *d = dst + item * dst_item_stride + (long long)comp * K * n + c;
     const u64 half = SP.p >> 1;
     const b200_u64x2 sp = ldg2(acc + (long long)K * n);
     u64 s0 = sp.x + half, s1 = sp.y + half;
@@ -454,14 +455,57 @@ __global__ void ksmoddown_kernel_v2(const PrimeDev *primes, int special_idx, con
         u64 v1 = a.y + (Q.p - barrett64(s1, Q.p, Q.r1)) + h;
         v0 = shoup_mul(v0, w, wq, Q.p);
         v1 = shoup_mul(v1, w, wq, Q.p);
-        if (base)
-        {
-            const b200_u64x2 b = ldg2(base + c + (long long)i * n);
-            v0 = add_mod(v0, b.x, Q.p);
-            v1 = add_mod(v1, b.y, Q.p);
-        }
-        stg2(d + (long long)i * n, v0, v1);
+        stg2(d + (long long)i * n, add_mod(v0, base[0][i], Q.p), add_mod(v1, base[1][i], Q.p));
     }
+}
+
+// ksmoddown_kernel with two adjacent coefficients per thread: 128-bit loads / stores (the kernel is a pure stream of
+// 2(k+1) + k rows in, 2k rows out per item)
+template <int K>
+__global__ void ksmoddown_kernel_v2(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *ks2,
+                                    const u64 *base0, long long base0_stride, const u64 *base1, long long base1_stride,
+                                    u64 *dst, long long dst_item_stride, long long n, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long hn = n >> 1;
+    const long long c = (idx % hn) * 2;
+    const long long t = idx / hn;
+    const int comp = (int)(t & 1);
+    const long long item = t >> 1;
+    const u64 *base = comp == 0 ? (base0 ? base0 + item * base0_stride : nullptr) : (base1 ? base1 + item * base1_stride : nullptr);
+    u64 b[2][K];
+#pragma unroll
+    for (int i = 0; i < K; i++)
+    {
+        const b200_u64x2 v = base ? ldg2(base + c + (long long)i * n) : b200_u64x2{ 0, 0 };
+        b[0][i] = v.x;
+        b[1][i] = v.y;
+    }
+    ksmoddown2<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, b,
+                  dst + item * dst_item_stride + (long long)comp * K * n + c);
+}
+
+// multiply_relin on the FP64 path: scale_kernel_v2 of the products D0, D1 fused into ksmoddown_kernel_v2 as its base, so that
+// c0 and c1 of the product never pass through HBM.  One thread per (item, component, two adjacent coefficients); D is
+// [item][3][k + |Bsk|][n] as multiply_core leaves it, dst [item][2][k][n].
+template <int K>
+__global__ void scale_moddown_kernel_v2(const ScaleFpC<K> L, const PrimeDev *primes, int special_idx, const u64 *inv_qsp,
+                                        const u64 *D, const u64 *ks2, u64 *dst, long long n, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long hn = n >> 1;
+    const long long c = (idx % hn) * 2;
+    const long long t = idx / hn;
+    const int comp = (int)(t & 1);
+    const long long item = t >> 1;
+    u64 b[2][K];
+    scale2_fp<K>(L, D + ((item * 3 + comp) * (K + L.nBsk)) * n + c, n, b);
+    ksmoddown2<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, b,
+                  dst + (item * 2 + comp) * K * n + c);
 }
 
 template <int K>
@@ -1596,8 +1640,10 @@ static std::vector<int> row_primes(b200_ctx *ctx, int level, bool with_bsk)
 }
 
 // ---- multiply core: writes polys [0,split) to dst0 and [split,Dn) to dst1 ----
+// keep_D (FP64 levels only): the caller's buffer of batch * Dn * (k + |Bsk|) * n words for the products D, which outlives the
+// call; polys [0, split) are then not scaled and stay in keep_D (dst0 unused) for scale_moddown_kernel_v2
 static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u64 *b, int sb, bool square, u64 *dst0,
-                         int split, u64 *dst1, long long batch, cudaStream_t s)
+                         int split, u64 *dst1, long long batch, cudaStream_t s, u64 *keep_D = nullptr)
 {
     const LevelDev &L = ctx->levels[level];
     const LevelHost &Lh = ctx->host->levels[level];
@@ -1606,11 +1652,11 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
     const int P = square ? sa : sa + sb;
     const int Dn = square ? 3 : sa + sb - 1;
     Scratch scr(ctx, s);
-    u64 *ext = nullptr, *D = nullptr;
+    u64 *ext = nullptr, *D = keep_D;
     int rc;
     if ((rc = scr.get((size_t)batch * P * R * n, &ext)))
         return rc;
-    if ((rc = scr.get((size_t)batch * Dn * R * n, &D)))
+    if (!D && (rc = scr.get((size_t)batch * Dn * R * n, &D)))
         return rc;
     bool clustered = false; // (3)-(5) ran as mul_cluster_kernel
     // (1)-(2) lift to Bsk
@@ -1755,9 +1801,10 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
     {
         if (L.fp)
         {
-            const long long total = batch * Dn * (n >> 1);
+            const int m0 = keep_D ? split : 0;
+            const long long total = batch * (Dn - m0) * (n >> 1);
             DISPATCH_K(k, B200_LAUNCH(scale_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, make_scale_fpc<KK>(ctx, level), D, Dn,
-                                      dst0, split, dst1, n, total));
+                                      m0, dst0, split, dst1, n, total));
         }
         else
         {
@@ -1772,9 +1819,11 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
 }
 
 // ---- key switch core: target d (k rows per item, stride d_stride), key list; dst_c = base_c + moddown(acc_c) ----
+// D (FP64 levels only; base0 / base1 unused): the unscaled products of multiply_core's keep_D; base_c = scale(D_c), formed in
+// the mod-down kernel; dst is then [item][2][k][n]
 static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_stride, const u64 *key, const u64 *base0,
                           long long base0_stride, const u64 *base1, long long base1_stride, u64 *dst,
-                          long long dst_stride, long long batch, cudaStream_t s)
+                          long long dst_stride, long long batch, cudaStream_t s, const u64 *D = nullptr)
 {
     if (!ctx->host->using_keyswitching || level < 1)
         return fail(B200_E_LOGIC, "keyswitching is not supported by the context");
@@ -1920,9 +1969,17 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
     }
     {
         const long long total = batch * 2 * (n >> 1);
-        DISPATCH_K(k, B200_LAUNCH(ksmoddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special, ctx->d_inv_qsp, ks2,
-                                                                                base0, base0_stride, base1, base1_stride,
-                                                                                dst, dst_stride, n, total));
+        if (D)
+        {
+            DISPATCH_K(k, B200_LAUNCH(scale_moddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, make_scale_fpc<KK>(ctx, level),
+                                      ctx->d_primes, special, ctx->d_inv_qsp, D, ks2, dst, n, total));
+        }
+        else
+        {
+            DISPATCH_K(k, B200_LAUNCH(ksmoddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special, ctx->d_inv_qsp, ks2,
+                                                                                    base0, base0_stride, base1, base1_stride,
+                                                                                    dst, dst_stride, n, total));
+        }
         ctx->launches++;
     }
     CU_TRY(cudaGetLastError());
@@ -2678,16 +2735,30 @@ static int multiply_relin_one(b200_ctx *ctx, int level, const uint64_t *a, const
         return 0;
     CU_TRY(cudaSetDevice(ctx->device));
     const long long n = (long long)ctx->n;
-    const int k = ctx->levels[level].k;
+    const LevelDev &L = ctx->levels[level];
+    const int k = L.k, R = k + L.nBsk;
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
-    u64 *c2 = nullptr;
+    u64 *c2 = nullptr, *D = nullptr;
     if ((rc = scr.get((size_t)batch * k * n, &c2)))
         return rc;
-    // c0,c1 go straight into out2; c2 into scratch
-    if ((rc = multiply_core(ctx, level, (const u64 *)a, 2, (const u64 *)b, 2, false, (u64 *)out2, 2, c2, (long long)batch, s)))
-        return rc;
     u64 *o = (u64 *)out2;
+    // FP64 levels: c0, c1 are scaled inside the key switch's mod-down (scale_moddown_kernel_v2), from the products D kept
+    // here, instead of going through out2 and back.  D (3R rows per item) then lives beside the key switch's scratch (at most
+    // k(k + 1) + 2(k + 1) rows), which stays within the multiply's own ext + D (7R) while (k + 1)(k + 2) <= 4R; above that
+    // (k = 7, 8 of the n = 16384 chain) the separate scale keeps the peak scratch where it was.
+    if (L.fp && (k + 1) * (k + 2) <= 4 * R)
+    {
+        if ((rc = scr.get((size_t)batch * 3 * R * n, &D)))
+            return rc;
+        if ((rc = multiply_core(ctx, level, (const u64 *)a, 2, (const u64 *)b, 2, false, nullptr, 2, c2, (long long)batch, s, D)))
+            return rc;
+        return keyswitch_core(ctx, level, c2, (long long)k * n, (const u64 *)relin_key, nullptr, 0, nullptr, 0, o, 2LL * k * n,
+                              (long long)batch, s, D);
+    }
+    // c0,c1 go straight into out2; c2 into scratch
+    if ((rc = multiply_core(ctx, level, (const u64 *)a, 2, (const u64 *)b, 2, false, o, 2, c2, (long long)batch, s)))
+        return rc;
     return keyswitch_core(ctx, level, c2, (long long)k * n, (const u64 *)relin_key, o, 2LL * k * n, o + (long long)k * n,
                           2LL * k * n, o, 2LL * k * n, (long long)batch, s);
 }
