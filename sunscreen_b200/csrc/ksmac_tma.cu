@@ -21,6 +21,7 @@ namespace
 {
 constexpr int TILE = 256; // coefficients per key tile (TMA box dimension limit)
 constexpr int NT = 128;   // threads: two adjacent coefficients each
+constexpr size_t STATIC_SMEM = 1024; // static shared memory of ksmac_tma_kernel (ptxas -v: the mbarrier, padded)
 
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 
@@ -167,17 +168,20 @@ int launch(bool fp, const CUtensorMap &tm, const PrimeDev *primes, const NttPrim
         ipc = (ipc + 1) / 2;
     const unsigned chunks = (unsigned)((batch + ipc - 1) / ipc);
     const size_t smem = 2 * (size_t)K * TILE * sizeof(u64);
+    // the 48 KiB a launch gets without opting in also holds the static mbarrier, which the 1024-byte alignment of the dynamic
+    // tile pads to 1024 bytes: at K = 12 the tile alone is 48 KiB, so the opt-in is needed from there on
+    const bool opt_in = smem + STATIC_SMEM > 48 * 1024;
     dim3 grid((unsigned)tiles, (unsigned)(K + 1), chunks);
     cudaError_t e;
     if (fp)
     {
-        if (smem > 48 * 1024 && (e = cudaFuncSetAttribute(ksmac_tma_kernel<K, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
+        if (opt_in && (e = cudaFuncSetAttribute(ksmac_tma_kernel<K, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
             return (int)e;
         ksmac_tma_kernel<K, true><<<grid, NT, smem, s>>>(tm, primes, fprimes, special_idx, key_rows, ks1, ks2, n, batch, (int)ipc);
     }
     else
     {
-        if (smem > 48 * 1024 && (e = cudaFuncSetAttribute(ksmac_tma_kernel<K, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
+        if (opt_in && (e = cudaFuncSetAttribute(ksmac_tma_kernel<K, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
             return (int)e;
         ksmac_tma_kernel<K, false><<<grid, NT, smem, s>>>(tm, primes, fprimes, special_idx, key_rows, ks1, ks2, n, batch, (int)ipc);
     }

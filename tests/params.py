@@ -62,6 +62,35 @@ PARAMS.update({
 SEC_NONE = {"n1024_2x27"}   # sets the reference must be created for without a security level
 EDGE = list(EDGE_BITS)
 
+# Long chains (also from CoeffModulus::Create): every cluster size of the key switch and up to 16 data residues on the FP64
+# path.  Kept out of EDGE, whose parametrisations they would slow down; tests/test_gpu_long_chains.py runs them.
+LONG_BITS = {
+    # data levels k = 8 ... 1 at logn 13: ks_cluster_kernel at every cluster size 2 ... 8, mul_cluster_kernel up to k + |Bsk| = 14,
+    # and both sides of multiply_relin's fused scale-and-mod-down rule
+    "n8192_9x24": (8192, [24] * 9),
+    # the same walk at logn 12 (two chunks per round in the cluster's inner product); 198 bits exceed 128-bit security at
+    # n = 4096 (SEC_NONE)
+    "n4096_9x22": (4096, [22] * 9),
+    # the special prime narrowest (21 bits: the 20-bit one Create hands out is t = 1032193 itself), a 49-bit data prime and so
+    # the 49-bit auxiliary base, k = 5 at the top: mixed widths inside one cluster job
+    "n8192_mixed_fp": (8192, [49, 36, 30, 30, 30, 21]),
+    # 16 data residues on the FP64 BEHZ and key-switch kernels (47-bit auxiliary base)
+    "n16384_17x25": (16384, [25] * 17),
+    # 16 data residues against 49-bit auxiliary primes: the FP64 inner products at their largest
+    "n16384_49_16x24": (16384, [49] + [24] * 16),
+}
+PARAMS.update({
+    "n8192_9x24": (8192, [0xf34001, 0xf3c001, 0xf60001, 0xf84001, 0xfa0001, 0xfb4001, 0xfc0001, 0xfd0001, 0xffc001], 1032193),
+    "n4096_9x22": (4096, [0x390001, 0x3ac001, 0x3c6001, 0x3d2001, 0x3dc001, 0x3e4001, 0x3ea001, 0x3ee001, 0x3fa001], 262144),
+    "n8192_mixed_fp": (8192, [0x1fffffff74001, 0xffffc4001, 0x3ffc0001, 0x3ffe8001, 0x3fff4001, 0x1b4001], 1032193),
+    "n16384_17x25": (16384, [0x1bf0001, 0x1c50001, 0x1c80001, 0x1cc8001, 0x1cf8001, 0x1d20001, 0x1d58001, 0x1d88001, 0x1de0001,
+                             0x1df8001, 0x1e70001, 0x1e78001, 0x1ef0001, 0x1f60001, 0x1f68001, 0x1f98001, 0x1fc0001], 786433),
+    "n16384_49_16x24": (16384, [0x1fffffff68001, 0xc18001, 0xc78001, 0xca0001, 0xcb8001, 0xcf0001, 0xd00001, 0xd08001, 0xd78001,
+                                0xd80001, 0xe38001, 0xe40001, 0xee8001, 0xf60001, 0xfa0001, 0xfc0001, 0xfd0001], 786433),
+})
+SEC_NONE.add("n4096_9x22")
+LONG = list(LONG_BITS)
+
 # Plain moduli beyond 20 bits on chains above: name -> (chain, how t is chosen).  A batching t is what
 # PlainModulus::Batching(n, bits) returns, the largest prime = 1 mod 2n below 2^bits (CoeffModulus::Create(n, {bits})),
 # skipping the chain's own primes where noted; tests/test_params.py re-derives each.

@@ -6,7 +6,7 @@ import math
 
 import pytest
 
-from params import EDGE, EDGE_BITS, PARAMS, PLAIN_EDGE, PLAIN_EDGE_T, SEC_NONE
+from params import EDGE, EDGE_BITS, LONG, LONG_BITS, PARAMS, PLAIN_EDGE, PLAIN_EDGE_T, SEC_NONE
 
 
 def is_prime(v):
@@ -85,6 +85,31 @@ def test_edge_chains_reach_their_cases():
         assert n == 1 << logn and len(m) == 2 and t % (2 * n) == 1
 
 
+@pytest.mark.parametrize("name", LONG)
+def test_long_chain_is_create_output(name):
+    n, bits = LONG_BITS[name]
+    _, moduli, t = PARAMS[name]
+    assert [q.bit_length() for q in moduli] == bits
+    assert moduli == create_coeff_modulus(n, bits)
+    assert t == {4096: 262144, 8192: 1032193, 16384: 786433}[n]     # the default plain modulus of each n
+
+
+def test_long_chains_reach_their_cases():
+    """What each long chain is there for (host_ctx.h: FP64 primes are <= 49 bits; the auxiliary base is as wide as the
+    widest user prime, at least 47 bits; b200_bfv.cu: the key-switch cluster runs 2 <= k <= 8 at logn 12 and 13)."""
+    assert all(q.bit_length() <= 49 for name in LONG for q in PARAMS[name][1])
+    for name, logn in (("n8192_9x24", 13), ("n4096_9x22", 12)):
+        n, m, t = PARAMS[name]
+        assert n == 1 << logn and len(m) - 1 == 8                      # data levels k = 8 ... 1
+    n, m, t = PARAMS["n8192_mixed_fp"]
+    assert m[-1] < min(m[:-1]) and max(q.bit_length() for q in m) == 49 and len({q.bit_length() for q in m[:-1]}) == 3
+    # the 20-bit prime Create would hand out as the special prime is the default t itself
+    assert create_coeff_modulus(n, [20]) == [t]
+    for name, widest in (("n16384_17x25", 25), ("n16384_49_16x24", 49)):
+        n, m, t = PARAMS[name]
+        assert len(m) - 1 == 16 and max(q.bit_length() for q in m) == widest
+
+
 def batching_plain_modulus(n, bits, skip=()):
     """PlainModulus::Batching(n, bits) = CoeffModulus::Create(n, {bits})[0], the largest prime = 1 mod 2n below 2^bits;
     with `skip`, the largest such prime not in it."""
@@ -145,10 +170,18 @@ def test_plain_edge_matches_reference(ref, name):
     refseal.RefContext(n, moduli, t)
 
 
+@pytest.mark.parametrize("name", LONG)
+def test_long_chain_matches_reference_create(ref, name):
+    reference_create_matches(ref, name, *LONG_BITS[name])
+
+
 @pytest.mark.parametrize("name", EDGE)
 def test_edge_chain_matches_reference_create(ref, name):
+    reference_create_matches(ref, name, *EDGE_BITS[name])
+
+
+def reference_create_matches(ref, name, n, bits):
     import refseal
-    n, bits = EDGE_BITS[name]
     arr = (C.c_int * len(bits))(*bits)
     out = (C.c_void_p * len(bits))()
     ref.call("CoeffModulus_Create1", C.c_uint64(n), C.c_uint64(len(bits)), arr, out)
