@@ -16,6 +16,8 @@
  *   b200_apply_galois    Evaluator_ApplyGalois / RotateRows / RotateColumns   -> apply_galois_inplace     S/evaluator.cpp:2221-2323
  *   b200_add/sub/negate  Evaluator_Add/Sub/Negate                             -> S/evaluator.cpp:130-350
  *   b200_multiply_plain  Evaluator_MultiplyPlain                              -> multiply_plain_normal    S/evaluator.cpp:1858-1992
+ *   b200_plain_to_ntt    Evaluator_TransformToNTT1                            -> transform_to_ntt_inplace S/evaluator.cpp:2033-2124
+ *   b200_multiply_plain_sum  a chain of multiply_plain + add_inplace (plaintext matrix x ciphertext vector)
  *   b200_add_plain / b200_sub_plain   Evaluator_AddPlain/SubPlain             -> S/util/scalingvariant.cpp:69-188
  *   b200_mod_switch_to_next           Evaluator_ModSwitchToNext1              -> S/util/rns.cpp:801-840
  *   b200_ntt_forward / b200_ntt_inverse  (util level)                         -> S/util/ntt.cpp:393-474
@@ -125,6 +127,19 @@ int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t ga
    (m + (Q - t) for m >= (t+1)/2).  The two are congruent mod t but give different ciphertext words. */
 int b200_multiply_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t plain_batch,
                         uint64_t *out, uint64_t batch, void *stream);
+/* plain: [pb][n] coefficients -> out: [pb][k][n] in NTT form at `level`.  `rule` selects the lift:
+     B200_PLAIN_NTT_TRANSFORM  Evaluator::transform_to_ntt_inplace(Plaintext &, parms_id) (S/evaluator.cpp:2033-2124): every
+                               coefficient m >= (t+1)/2 becomes m + (Q - t)
+     B200_PLAIN_NTT_MULTIPLY   the operand b200_multiply_plain multiplies by, monomial path included (S/evaluator.cpp:1885-1933)
+   The two differ only for a monomial with its coefficient in the upper half under the fast plain lift (every q_i > t). */
+#define B200_PLAIN_NTT_TRANSFORM 0
+#define B200_PLAIN_NTT_MULTIPLY 1
+int b200_plain_to_ntt(b200_ctx *ctx, int level, const uint64_t *plain, uint64_t pb, uint64_t *out, int rule, void *stream);
+/* plaintext matrix x ciphertext vector: out[i] = sum_{j<m} multiply_plain(cts[j], plain i,j) for i < R, word for word.
+   cts: [m][size][k][n] coefficient form; plain_ntt: [R][m][k][n] from b200_plain_to_ntt; out: [R][size][k][n], must not
+   overlap cts.  Each ciphertext is transformed once and each output once; m or R = 0 is a no-op. */
+int b200_multiply_plain_sum(b200_ctx *ctx, int level, const uint64_t *cts, int size, uint64_t m, const uint64_t *plain_ntt,
+                            uint64_t R, uint64_t *out, void *stream);
 int b200_add_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t plain_batch,
                    uint64_t *out, uint64_t batch, void *stream);
 int b200_sub_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t plain_batch,

@@ -284,6 +284,12 @@ SEAL_C_FUNC B200_Evaluator_PlainBatch(void *thisptr, int which, uint64_t count, 
 /* one row rotation for all items; the Galois key for `steps` must be present */
 SEAL_C_FUNC B200_Evaluator_RotateRowsBatch(void *thisptr, uint64_t count, void **encrypteds, int steps, void *galois_keys,
                                            void **destinations);
+/* plaintext matrix x ciphertext vector: destinations[i] receives the words of multiply_plain(encrypteds[0], plains[i*cols])
+   followed by add_inplace(multiply_plain(encrypteds[j], plains[i*cols + j])) for j = 1 ... cols-1 (plains row-major,
+   rows x cols).  Same checks and HRESULTs as those calls, except: all encrypteds must have one size, and a transparent
+   partial sum is not detected (only a transparent final result).  Destinations may alias encrypteds. */
+SEAL_C_FUNC B200_Evaluator_MultiplyPlainSum(void *thisptr, uint64_t rows, uint64_t cols, void **encrypteds, void **plains,
+                                            void **destinations);
 
 #ifdef __cplusplus
 }

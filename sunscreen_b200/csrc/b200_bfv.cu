@@ -595,6 +595,77 @@ __global__ void dyadic_plain_kernel(const PrimeDev *primes, int k, int size, con
     out[idx] = barrett128(lo, hi, P.p, P.r0, P.r1);
 }
 
+// Plaintext-matrix x ciphertext-vector product in the NTT domain (b200_multiply_plain_sum):
+//     out[i][c][r][x] = sum_{j<m} X[j][c][r][x] * P[i][j][r][x] mod q_r      X: [m][size][k][n], P: [R][m][k][n], canonical
+// for the polys [c0, c0 + SZ) of each ciphertext.  The pass is bound by reading P, which every output row reads once: a thread
+// owns one coefficient pair (128-bit loads) of one residue for MAC_ROWS output rows, so each X pair it loads serves MAC_ROWS
+// rows.  blockIdx.x runs over row blocks, so the CTAs resident at one time share their X tile and X comes from HBM about
+// once.  Products of canonical words are below q^2 and are summed lazily in 128 bits; `lazy` (at most 256, fewer for primes
+// over 60 bits, b200_multiply_plain_sum) bounds the terms between two reductions so that the sum never wraps.
+#define MAC_ROWS 4
+#define MAC_NT 256
+template <int SZ>
+__global__ void __launch_bounds__(MAC_NT) plain_mac_kernel(const PrimeDev *primes, int k, int size, int c0, const u64 *X,
+                                                           const u64 *P, long long m, long long R, int lazy, u64 *out, int logn)
+{
+    const long long kn = (long long)k << logn;
+    const long long off = ((long long)blockIdx.y * blockDim.x + threadIdx.x) * 2; // r * n + x of the pair
+    if (off >= kn)
+        return;
+    const PrimeDev Q = ld_prime(&primes[(int)(off >> logn)]);
+    const long long i0 = (long long)blockIdx.x * MAC_ROWS;
+    const long long xs = (long long)size * kn; // one ciphertext
+    u64 lo[MAC_ROWS][SZ][2], hi[MAC_ROWS][SZ][2];
+#pragma unroll
+    for (int u = 0; u < MAC_ROWS; u++)
+#pragma unroll
+        for (int c = 0; c < SZ; c++)
+            lo[u][c][0] = lo[u][c][1] = hi[u][c][0] = hi[u][c][1] = 0;
+    for (long long j0 = 0; j0 < m; j0 += lazy)
+    {
+        const long long j1 = j0 + lazy < m ? j0 + lazy : m;
+        for (long long j = j0; j < j1; j++)
+        {
+            b200_u64x2 x[SZ];
+#pragma unroll
+            for (int c = 0; c < SZ; c++)
+                x[c] = ldg2(X + j * xs + (c0 + c) * kn + off);
+#pragma unroll
+            for (int u = 0; u < MAC_ROWS; u++)
+            {
+                if (i0 + u >= R)
+                    break;
+                const b200_u64x2 p = ldg2(P + ((i0 + u) * m + j) * kn + off);
+#pragma unroll
+                for (int c = 0; c < SZ; c++)
+                {
+                    mac128(x[c].x, p.x, lo[u][c][0], hi[u][c][0]);
+                    mac128(x[c].y, p.y, lo[u][c][1], hi[u][c][1]);
+                }
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < MAC_ROWS; u++)
+#pragma unroll
+            for (int c = 0; c < SZ; c++)
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+                {
+                    lo[u][c][h] = barrett128(lo[u][c][h], hi[u][c][h], Q.p, Q.r0, Q.r1);
+                    hi[u][c][h] = 0;
+                }
+    }
+#pragma unroll
+    for (int u = 0; u < MAC_ROWS; u++)
+    {
+        if (i0 + u >= R)
+            break;
+#pragma unroll
+        for (int c = 0; c < SZ; c++)
+            stg2(out + ((i0 + u) * size + c0 + c) * kn + off, lo[u][c][0], lo[u][c][1]);
+    }
+}
+
 // mono[item] = 1 when plaintext `item` has exactly one nonzero coefficient (the monomial test of multiply_plain_normal,
 // S/evaluator.cpp:1885).  One block per item: strided per-thread counts, summed in shared memory (blockDim a power of 2).
 // The CPU emulation build runs kernels with dynamic shared memory as one thread per block, so only the CUDA build executes
@@ -2820,6 +2891,37 @@ int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t ga
                           2LL * k * n, (long long)batch, s);
 }
 
+// plain [pb][n] -> out [pb][k][n]: each plaintext lifted to the level's residues and put in NTT form.  monomial != 0 gives
+// the operand multiply_plain_normal multiplies by, with its monomial path (S/evaluator.cpp:1885-1933); monomial == 0 the
+// upper-half lift of transform_to_ntt_inplace(Plaintext &, parms_id) (S/evaluator.cpp:2033-2124).
+static int plain_lift_ntt(b200_ctx *ctx, int level, const u64 *plain, uint64_t pb, u64 *out, bool monomial, Scratch &scr,
+                          cudaStream_t s)
+{
+    int rc;
+    const long long n = (long long)ctx->n;
+    const LevelDev &L = ctx->levels[level];
+    const int k = L.k;
+    u32 *mono = nullptr;
+    if (monomial && L.fast_plain_lift)
+    {
+        u64 *flags = nullptr;
+        if ((rc = scr.get((size_t)(pb + 1) / 2, &flags)))
+            return rc;
+        mono = (u32 *)flags;
+        B200_LAUNCH(plain_monomial_kernel, (unsigned)pb, 1024, 1024 * sizeof(u64), s, plain, n, mono);
+        ctx->launches++;
+    }
+    {
+        const long long total = (long long)pb * k * n;
+        B200_LAUNCH(plain_lift_kernel, blocks_for(total, EB), EB, 0, s, L, plain, (const u32 *)mono, out, ctx->logn, total);
+        ctx->launches++;
+    }
+    JobDesc jd;
+    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+        return rc;
+    return launch_ntt<true>(ctx, jd, out, (long long)k * n, out, (long long)k * n, (long long)pb, 0, s);
+}
+
 int b200_multiply_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t pb,
                         uint64_t *out, uint64_t batch, void *stream)
 {
@@ -2834,33 +2936,16 @@ int b200_multiply_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, c
         return 0;
     CU_TRY(cudaSetDevice(ctx->device));
     const long long n = (long long)ctx->n;
-    const LevelDev &L = ctx->levels[level];
-    const int k = L.k;
+    const int k = ctx->levels[level].k;
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
     u64 *pl = nullptr;
     if ((rc = scr.get((size_t)pb * k * n, &pl)))
         return rc;
-    u32 *mono = nullptr;
-    if (L.fast_plain_lift)
-    {
-        u64 *flags = nullptr;
-        if ((rc = scr.get((size_t)(pb + 1) / 2, &flags)))
-            return rc;
-        mono = (u32 *)flags;
-        B200_LAUNCH(plain_monomial_kernel, (unsigned)pb, 1024, 1024 * sizeof(u64), s, (const u64 *)plain, n, mono);
-        ctx->launches++;
-    }
-    {
-        const long long total = (long long)pb * k * n;
-        B200_LAUNCH(plain_lift_kernel, blocks_for(total, EB), EB, 0, s, L, (const u64 *)plain, (const u32 *)mono, pl, ctx->logn,
-                                                                total);
-        ctx->launches++;
-    }
+    if ((rc = plain_lift_ntt(ctx, level, (const u64 *)plain, pb, pl, true, scr, s)))
+        return rc;
     JobDesc jd;
     if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
-        return rc;
-    if ((rc = launch_ntt<true>(ctx, jd, pl, (long long)k * n, pl, (long long)k * n, (long long)pb, 0, s)))
         return rc;
     // ct polys: forward (out of place), dyadic, inverse
     if ((rc = launch_ntt<true>(ctx, jd, (const u64 *)a, (long long)k * n, (u64 *)out, (long long)k * n, (long long)batch * size, 0,
@@ -2874,6 +2959,90 @@ int b200_multiply_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, c
     }
     if ((rc = launch_ntt<false>(ctx, jd, (const u64 *)out, (long long)k * n, (u64 *)out, (long long)k * n,
                                 (long long)batch * size, 0, s)))
+        return rc;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+int b200_plain_to_ntt(b200_ctx *ctx, int level, const uint64_t *plain, uint64_t pb, uint64_t *out, int rule, void *stream)
+{
+    int rc = check_level(ctx, level);
+    if (rc)
+        return rc;
+    if (!plain || !out)
+        return fail(B200_E_NULL, "null pointer");
+    if (rule != B200_PLAIN_NTT_TRANSFORM && rule != B200_PLAIN_NTT_MULTIPLY)
+        return fail(B200_E_INVALID, "rule");
+    if (pb == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    if ((rc = plain_lift_ntt(ctx, level, (const u64 *)plain, pb, (u64 *)out, rule == B200_PLAIN_NTT_MULTIPLY, scr, s)))
+        return rc;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// Sums of multiply_plain products: out[i] = INTT(sum_j NTT(cts[j]) (*) plain_ntt[i][j]).  The inverse NTT is linear mod q and
+// every hand-off is canonical, so the words equal those of multiply_plain(cts[0], p_i0) + ... + multiply_plain(cts[m-1], ...)
+// while each ciphertext is transformed once and each output once.
+int b200_multiply_plain_sum(b200_ctx *ctx, int level, const uint64_t *cts, int size, uint64_t m, const uint64_t *plain_ntt,
+                            uint64_t R, uint64_t *out, void *stream)
+{
+    int rc = check_level(ctx, level);
+    if (rc)
+        return rc;
+    if (!cts || !plain_ntt || !out)
+        return fail(B200_E_NULL, "null pointer");
+    if (size < 1)
+        return fail(B200_E_INVALID, "size");
+    if (m == 0 || R == 0)
+        return 0;
+    const long long n = (long long)ctx->n;
+    const LevelHost &Lh = ctx->host->levels[level];
+    const int k = Lh.k;
+    const long long kn = (long long)k * n;
+    {
+        const uintptr_t x0 = (uintptr_t)cts, x1 = x0 + (uintptr_t)(m * size * kn * sizeof(u64));
+        const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (uintptr_t)(R * size * kn * sizeof(u64));
+        if (x0 < o1 && o0 < x1)
+            return fail(B200_E_INVALID, "out must not overlap cts");
+    }
+    CU_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    u64 *X = nullptr;
+    if ((rc = scr.get((size_t)m * size * kn, &X)))
+        return rc;
+    JobDesc jd;
+    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+        return rc;
+    if ((rc = launch_ntt<true>(ctx, jd, (const u64 *)cts, kn, X, kn, (long long)m * size, 0, s)))
+        return rc;
+    // terms between two reductions: r + lazy (q - 1)^2 < 2^128 for a remainder r < q of the previous chunk
+    int bits = 0;
+    for (int r = 0; r < k; r++)
+    {
+        const u64 q = ctx->host->primes[Lh.q_idx[r]].mod.p;
+        bits = std::max(bits, 64 - __builtin_clzll(q));
+    }
+    const int lazy = bits <= 60 ? 256 : 1 << (128 - 2 * bits);
+    const dim3 grid((unsigned)((R + MAC_ROWS - 1) / MAC_ROWS), blocks_for(kn / 2, MAC_NT));
+    for (int c0 = 0; c0 < size; c0 += 3)
+    {
+        const int sz = std::min(3, size - c0);
+        void (*kfn)(const PrimeDev *, int, int, int, const u64 *, const u64 *, long long, long long, int, u64 *, int) =
+            sz == 1 ? plain_mac_kernel<1> : sz == 2 ? plain_mac_kernel<2> : plain_mac_kernel<3>;
+#ifndef B200_EMU_HEADER
+        if (trace_on())
+            g_trace_name = "plain_mac_kernel";
+#endif
+        B200_LAUNCH(kfn, grid, MAC_NT, 0, s, ctx->d_primes, k, size, c0, X, (const u64 *)plain_ntt, (long long)m, (long long)R, lazy,
+                    (u64 *)out, ctx->logn);
+        ctx->launches++;
+    }
+    if ((rc = launch_ntt<false>(ctx, jd, (u64 *)out, kn, (u64 *)out, kn, (long long)R * size, 0, s)))
         return rc;
     CU_TRY(cudaGetLastError());
     return 0;

@@ -2046,18 +2046,19 @@ int batch_gather(Context_ *c, uint64_t count, void **cts, BatchSlab &slab, u64 &
     k_out = a0.k;
     return lv;
 }
-void batch_scatter(Context_ *c, uint64_t count, void **dsts, const BatchSlab &slab, const ParmsId &id, u64 k, int level)
+void batch_scatter(Context_ *c, uint64_t count, void **dsts, const BatchSlab &slab, const ParmsId &id, u64 k, int level,
+                   u64 size = 2)
 {
-    const u64 w = 2 * k * c->parms.n;
+    const u64 w = size * k * c->parms.n;
     std::vector<u64 *> ptrs(count);
     for (uint64_t i = 0; i < count; i++)
-        ptrs[i] = ((Ciphertext_ *)dsts[i])->prepare_output(c, id, 2, k);
+        ptrs[i] = ((Ciphertext_ *)dsts[i])->prepare_output(c, id, size, k);
     dev_check(b200_gather_scatter(c->dev, ptrs.data(), count, slab.w(), w, 0, cur_stream()));
     if (c->check_transparent)
     { // one flag per item
         BatchSlab flags(c, count);
         std::vector<uint32_t> h(count);
-        dev_check(b200_is_transparent(c->dev, level, slab.w(), 2, (uint32_t *)flags.p, count, cur_stream()));
+        dev_check(b200_is_transparent(c->dev, level, slab.w(), (int)size, (uint32_t *)flags.p, count, cur_stream()));
         dev_check(b200_memcpy_d2h(c->dev, h.data(), flags.p, count * 4, cur_stream()));
         tl_scope->wait(); // releases the context mutex while the batch completes
         for (uint32_t f : h)
@@ -2269,6 +2270,72 @@ long B200_Evaluator_RotateRowsBatch(void *p, uint64_t count, void **encs, int st
         check_keys(c, keys, index);
         dev_check(b200_apply_galois(c->dev, lv, A.w(), elt, keys.flat_dev(c, index, (int)k), O.w(), count, cur_stream()));
         batch_scatter(c, count, dsts, O, ((Ciphertext_ *)encs[0])->parms_id, k, lv);
+    });
+}
+// Plaintext matrix x ciphertext vector: destinations[i] <- the words of multiply_plain(encrypteds[0], plains[i * cols]) followed
+// by add_inplace(multiply_plain(encrypteds[j], plains[i * cols + j])) for j = 1 ... cols - 1.  The ciphertexts are gathered
+// once; the plaintexts go through b200_plain_to_ntt (multiply rule) in chunks of rows whose NTT-form scratch stays below
+// B200_PLAIN_SUM_SCRATCH bytes (default 1 GiB), each chunk one b200_multiply_plain_sum.  Every operand is read before the
+// first scatter, so destinations may alias encrypteds.
+long B200_Evaluator_MultiplyPlainSum(void *p, uint64_t rows, uint64_t cols, void **encs, void **plains, void **dsts)
+{
+    NULLRET(p);
+    NULLRET(encs);
+    NULLRET(plains);
+    NULLRET(dsts);
+    auto *c = ((Evaluator_ *)p)->ctx;
+    return guard([&] {
+        if (rows == 0)
+            return;
+        if (cols == 0)
+            throw InvalidArg("a sum needs at least one term");
+        batch_handles(cols, { encs });
+        batch_handles(rows, { dsts });
+        batch_handles(rows * cols, { plains });
+        OpScope scope(c);
+        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        const size_t n = c->parms.n;
+        auto &a0 = *(Ciphertext_ *)encs[0];
+        const int lv = data_level(c, a0, "encrypted is not valid for encryption parameters");
+        const u64 size = a0.size, k = a0.k, w = size * k * n;
+        const ParmsId id = a0.parms_id;
+        std::vector<u64 *> ptrs(cols);
+        for (uint64_t j = 0; j < cols; j++)
+        {
+            auto &a = *(Ciphertext_ *)encs[j];
+            if (data_level(c, a, "encrypted is not valid for encryption parameters") != lv)
+                throw InvalidArg("encrypted1 and encrypted2 parameter mismatch");
+            if (a.is_ntt_form)
+                throw InvalidArg("BFV encrypted cannot be in NTT form");
+            if (a.size != size)
+                throw InvalidArg("all encrypteds must have the same size");
+            ptrs[j] = const_cast<u64 *>(a.dev_ptr(c));
+        }
+        // the plaintext checks of the chain's multiply_plain, all before any work
+        std::vector<u64> host(rows * cols * n);
+        for (uint64_t i = 0; i < rows * cols; i++)
+        {
+            std::vector<u64> pv = padded_plain(c, *(Plaintext_ *)plains[i], false);
+            if (c->check_transparent && std::all_of(pv.begin(), pv.end(), [](u64 x) { return x == 0; }))
+                throw LogicErr("result ciphertext is transparent");
+            std::copy(pv.begin(), pv.end(), host.begin() + i * n);
+        }
+        BatchSlab X(c, cols * w);
+        dev_check(b200_gather_scatter(c->dev, ptrs.data(), cols, X.w(), w, 1, cur_stream()));
+        uint64_t cap = 1ull << 30;
+        if (const char *e = std::getenv("B200_PLAIN_SUM_SCRATCH"))
+            cap = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
+        const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(rows, cap / (cols * k * n * sizeof(u64))));
+        BatchSlab Pc(c, chunk * cols * n), Pn(c, chunk * cols * k * n), O(c, chunk * w);
+        for (uint64_t i0 = 0; i0 < rows; i0 += chunk)
+        {
+            const uint64_t r = std::min(chunk, rows - i0);
+            dev_check(b200_memcpy_h2d(c->dev, Pc.p, host.data() + i0 * cols * n, r * cols * n * sizeof(u64), cur_stream()));
+            dev_check(b200_plain_to_ntt(c->dev, lv, Pc.w(), r * cols, Pn.w(), B200_PLAIN_NTT_MULTIPLY, cur_stream()));
+            dev_check(b200_multiply_plain_sum(c->dev, lv, X.w(), (int)size, cols, Pn.w(), r, O.w(), cur_stream()));
+            scope.wait(); // `host` is read by the copy above
+            batch_scatter(c, r, dsts + i0, O, id, k, lv, size);
+        }
     });
 }
 

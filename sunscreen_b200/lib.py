@@ -12,6 +12,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200bfv.so")
 
 B200_OK, B200_E_INVALID, B200_E_LOGIC, B200_E_CUDA, B200_E_NULL, B200_E_NOMEM = 0, -1, -2, -3, -4, -5
+# lift rules of b200_plain_to_ntt
+PLAIN_NTT_TRANSFORM, PLAIN_NTT_MULTIPLY = 0, 1
 
 vp = C.c_void_p
 u64 = C.c_uint64
@@ -73,6 +75,8 @@ _SIGS = {
     "b200_multiply_relin": [vp, C.c_int, vp, vp, vp, vp, u64, vp],
     "b200_apply_galois": [vp, C.c_int, vp, C.c_uint32, vp, vp, u64, vp],
     "b200_multiply_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
+    "b200_plain_to_ntt": [vp, C.c_int, vp, u64, vp, C.c_int, vp],
+    "b200_multiply_plain_sum": [vp, C.c_int, vp, C.c_int, u64, vp, u64, vp, vp],
     "b200_add_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
     "b200_sub_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
     "b200_mod_switch_to_next": [vp, C.c_int, vp, C.c_int, vp, u64, vp],
@@ -258,6 +262,17 @@ class B200Context:
     def multiply_plain(self, a, size, plain, plain_batch, out, batch, level=None, stream=None):
         self.L.call("b200_multiply_plain", self.h, self._lv(level), vp(ptr(a)), C.c_int(size), vp(ptr(plain)),
                     u64(plain_batch), vp(ptr(out)), u64(batch), vp(stream))
+
+    def plain_to_ntt(self, plain, plain_batch, out, rule=PLAIN_NTT_TRANSFORM, level=None, stream=None):
+        """plain [plain_batch][n] -> out [plain_batch][k][n] in NTT form (rule: PLAIN_NTT_TRANSFORM or PLAIN_NTT_MULTIPLY)."""
+        self.L.call("b200_plain_to_ntt", self.h, self._lv(level), vp(ptr(plain)), u64(plain_batch), vp(ptr(out)), C.c_int(rule),
+                    vp(stream))
+
+    def multiply_plain_sum(self, cts, size, m, plain_ntt, R, out, level=None, stream=None):
+        """out[i] = sum_j multiply_plain(cts[j], plain i,j): cts [m][size][k][n], plain_ntt [R][m][k][n] from plain_to_ntt,
+        out [R][size][k][n]."""
+        self.L.call("b200_multiply_plain_sum", self.h, self._lv(level), vp(ptr(cts)), C.c_int(size), u64(m), vp(ptr(plain_ntt)),
+                    u64(R), vp(ptr(out)), vp(stream))
 
     def add_plain(self, a, size, plain, plain_batch, out, batch, level=None, stream=None):
         self.L.call("b200_add_plain", self.h, self._lv(level), vp(ptr(a)), C.c_int(size), vp(ptr(plain)), u64(plain_batch),
