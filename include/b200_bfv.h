@@ -14,6 +14,7 @@
  *   b200_square          Evaluator_Square          S/c/evaluator.cpp          -> Evaluator::bfv_square    S/evaluator.cpp:864-1020
  *   b200_relinearize     Evaluator_Relinearize     S/c/evaluator.cpp:333      -> relinearize_internal     S/evaluator.cpp:1104-1159
  *   b200_apply_galois    Evaluator_ApplyGalois / RotateRows / RotateColumns   -> apply_galois_inplace     S/evaluator.cpp:2221-2323
+ *   b200_apply_galois_add    apply_galois_inplace + add_inplace (one step of a rotate-and-sum reduction)
  *   b200_add/sub/negate  Evaluator_Add/Sub/Negate                             -> S/evaluator.cpp:130-350
  *   b200_multiply_plain  Evaluator_MultiplyPlain                              -> multiply_plain_normal    S/evaluator.cpp:1858-1992
  *   b200_plain_to_ntt    Evaluator_TransformToNTT1                            -> transform_to_ntt_inplace S/evaluator.cpp:2033-2124
@@ -121,6 +122,12 @@ int b200_multiply_relin(b200_ctx *ctx, int level, const uint64_t *a, const uint6
 /* size-2 cts: out = (sigma_g(c0), 0) + KeySwitch(sigma_g(c1), galois_key) */
 int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
                       uint64_t *out2, uint64_t batch, void *stream);
+/* out = addend + apply_galois(in): the words of b200_apply_galois followed by b200_add (apply_galois + add_inplace), with the
+   automorphism applied inside the key switch's digit loads and mod-down and the add folded into the mod-down.  addend2 ==
+   NULL: no addend (the words of b200_apply_galois).  addend2 may equal in2 or out2; out2 must not overlap in2.  One step of a
+   rotate-and-sum slot reduction (c = c + rotate_rows(c, s)). */
+int b200_apply_galois_add(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
+                          const uint64_t *addend2, uint64_t *out2, uint64_t batch, void *stream);
 /* plain: [batch or 1][n] coefficients mod t (plain_batch = 1 broadcasts one plaintext to every item).  multiply_plain
    follows the reference per plaintext item: an item with exactly one nonzero coefficient m is multiplied by m itself
    (its monomial path); any other item, and a monomial item when some q_i <= t, by the lifted plaintext

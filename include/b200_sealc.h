@@ -290,6 +290,14 @@ SEAL_C_FUNC B200_Evaluator_RotateRowsBatch(void *thisptr, uint64_t count, void *
    partial sum is not detected (only a transparent final result).  Destinations may alias encrypteds. */
 SEAL_C_FUNC B200_Evaluator_MultiplyPlainSum(void *thisptr, uint64_t rows, uint64_t cols, void **encrypteds, void **plains,
                                             void **destinations);
+/* rotate-and-sum slot reduction: destinations[i] receives the words of
+       c = encrypteds[i]; for s in steps: c = Evaluator_Add(c, Evaluator_RotateRows(c, s));
+       if columns: c = Evaluator_Add(c, Evaluator_RotateColumns(c))
+   Steps follow RotateRows: 0 adds c to itself, a step without its own key goes through its NAF parts.  Same checks and
+   HRESULTs as that chain, except that a transparent intermediate is not detected (only a transparent final result; a
+   transparent input stays transparent).  All encrypteds at one level; destinations may alias encrypteds. */
+SEAL_C_FUNC B200_Evaluator_RotateSumBatch(void *thisptr, uint64_t count, void **encrypteds, int nsteps, const int *steps, bool columns,
+                                          void *galois_keys, void **destinations);
 
 #ifdef __cplusplus
 }

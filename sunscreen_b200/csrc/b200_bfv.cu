@@ -508,6 +508,45 @@ __global__ void scale_moddown_kernel_v2(const ScaleFpC<K> L, const PrimeDev *pri
                   dst + (item * 2 + comp) * K * n + c);
 }
 
+// b200_apply_galois_add's mod-down: ksmoddown_kernel_v2 with the bases base_0 = addend_0 + sigma_g(in_0), base_1 = addend_1
+// (addend2 == nullptr: zero).  Canonical words summed mod q_i give one result for any grouping, so dst = addend +
+// apply_galois(in) word for word.  sigma_g(in_0) is gathered from in's c0 row: destination coefficient c takes source
+// i = c g^-1 mod 2n (ginv = g^-1), negated mod q_i where i >= n.  addend2 may be dst2 (each thread reads its words before it
+// writes them) or in2.  One thread per (item, component, two adjacent coefficients); in2, addend2, dst2 are [item][2][K][n].
+template <int K>
+__global__ void ksmoddown_galois_add_kernel(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *ks2,
+                                            const u64 *in2, const u64 *addend2, u64 *dst2, int logn, u32 ginv, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long n = 1LL << logn;
+    const long long hn = n >> 1;
+    const long long c = (idx % hn) * 2;
+    const long long t = idx / hn;
+    const int comp = (int)(t & 1);
+    const long long item = t >> 1;
+    const long long off = (item * 2 + comp) * K * n; // this component's rows in in2 / addend2 / dst2
+    const u64 m2 = 2 * (u64)n - 1, i0 = ((u64)c * ginv) & m2, i1 = ((u64)(c + 1) * ginv) & m2;
+    u64 b[2][K];
+#pragma unroll
+    for (int i = 0; i < K; i++)
+    {
+        b200_u64x2 v = addend2 ? ldg2(addend2 + off + (long long)i * n + c) : b200_u64x2{ 0, 0 };
+        if (comp == 0)
+        {
+            const u64 p = __ldg(&primes[i].p);
+            const u64 *row = in2 + off + (long long)i * n;
+            const u64 s0 = __ldg(row + (i0 & (n - 1))), s1 = __ldg(row + (i1 & (n - 1)));
+            v.x = add_mod(v.x, (i0 >> logn) ? neg_mod(s0, p) : s0, p);
+            v.y = add_mod(v.y, (i1 >> logn) ? neg_mod(s1, p) : s1, p);
+        }
+        b[0][i] = v.x;
+        b[1][i] = v.y;
+    }
+    ksmoddown2<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, b, dst2 + off + c);
+}
+
 template <int K>
 __global__ void modswitch_kernel(const PrimeDev *primes, const u64 *inv_qlast, const u64 *src, u64 *dst, long long n,
                                  long long total)
@@ -520,7 +559,8 @@ __global__ void modswitch_kernel(const PrimeDev *primes, const u64 *inv_qlast, c
     modswitch_coeff<K>(primes, inv_qlast, src + poly * K * n, n, dst + poly * (K - 1) * n, c);
 }
 
-// out0 <- sigma(c0) (into dst poly 0), tmp <- sigma(c1)
+// out0 <- sigma(c0) (into dst poly 0), tmp <- sigma(c1); out2 == nullptr: tmp <- sigma(c1) only (total = batch k n), for the
+// key switch of b200_apply_galois_add, whose mod-down gathers sigma(c0) itself
 __global__ void galois_kernel(const PrimeDev *primes, int k, const u64 *in2, u64 *out2, u64 *tmp, int logn, u32 g,
                               long long total)
 {
@@ -532,8 +572,8 @@ __global__ void galois_kernel(const PrimeDev *primes, int k, const u64 *in2, u64
     const long long t = idx >> logn;
     const int r = (int)(t % k);
     const long long u = t / k;
-    const int poly = (int)(u & 1);
-    const long long item = u >> 1;
+    const int poly = out2 ? (int)(u & 1) : 1;
+    const long long item = out2 ? u >> 1 : u;
     const u64 p = __ldg(&primes[r].p);
     const u64 *src = in2 + ((item * 2 + poly) * k + r) * n;
     u64 *dst = poly == 0 ? out2 + ((item * 2) * k + r) * n : tmp + (item * k + r) * n;
@@ -1889,12 +1929,23 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
     return 0;
 }
 
+// b200_apply_galois_add through keyswitch_core: the target is sigma_g(c1) of in2 [item][2][k][n], dst = addend2 + apply_galois(in2)
+struct KsGalois
+{
+    const u64 *in2, *addend2; // addend2 == nullptr: no addend
+    u32 g, ginv;              // the Galois element and its inverse mod 2n
+};
+
 // ---- key switch core: target d (k rows per item, stride d_stride), key list; dst_c = base_c + moddown(acc_c) ----
 // D (FP64 levels only; base0 / base1 unused): the unscaled products of multiply_core's keep_D; base_c = scale(D_c), formed in
 // the mod-down kernel; dst is then [item][2][k][n]
+// gal (d, d_stride, base0 / base1 unused): the rotate-add of KsGalois.  The cluster kernel gathers sigma_g(c1) in its digit loads;
+// otherwise galois_kernel writes sigma_g(c1) alone to scratch for the separate kernels.  The mod-down gathers sigma_g(c0) and adds
+// the addend (ksmoddown_galois_add_kernel); dst is then [item][2][k][n]
 static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_stride, const u64 *key, const u64 *base0,
                           long long base0_stride, const u64 *base1, long long base1_stride, u64 *dst,
-                          long long dst_stride, long long batch, cudaStream_t s, const u64 *D = nullptr)
+                          long long dst_stride, long long batch, cudaStream_t s, const u64 *D = nullptr,
+                          const KsGalois *gal = nullptr)
 {
     if (!ctx->host->using_keyswitching || level < 1)
         return fail(B200_E_LOGIC, "keyswitching is not supported by the context");
@@ -1909,6 +1960,11 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
     int rc;
     if ((rc = scr.get((size_t)batch * 2 * (k + 1) * n, &ks2)))
         return rc;
+    if (gal)
+    {
+        d = gal->in2 + (long long)k * n;
+        d_stride = 2LL * k * n;
+    }
     bool clustered = false; // the forward NTTs, the inner product and the inverse NTTs ran as ks_cluster_kernel
 #ifndef B200_EMU_HEADER
     // all three in one kernel on the FP64 static path (mul_cluster.cu): the transformed digits and the accumulators stay in the
@@ -1944,13 +2000,14 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
                 cudaEventCreate(&t1);
                 cudaEventRecord(t0, s);
             }
-            const int crc = b200_ks_cluster(ctx->logn, job, d, d_stride, key, Kkey, ks2, k, s);
+            const char *kname = gal ? "ks_cluster_galois_kernel" : "ks_cluster_kernel";
+            const int crc = b200_ks_cluster(ctx->logn, job, d, d_stride, key, Kkey, ks2, k, gal ? gal->ginv : 0u, s);
             if (crc)
-                return fail(B200_E_CUDA, std::string("ks_cluster_kernel: ") + cudaGetErrorString((cudaError_t)crc));
+                return fail(B200_E_CUDA, std::string(kname) + ": " + cudaGetErrorString((cudaError_t)crc));
             if (t0)
             {
                 cudaEventRecord(t1, s);
-                g_trace.push_back(B200TraceRec{ "ks_cluster_kernel", t0, t1 });
+                g_trace.push_back(B200TraceRec{ kname, t0, t1 });
             }
             ctx->launches++;
             clustered = true;
@@ -1959,6 +2016,18 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
 #endif
     if (!clustered && (rc = scr.get((size_t)batch * (k + 1) * k * n, &ks1)))
         return rc;
+    if (!clustered && gal)
+    {
+        u64 *sc1 = nullptr;
+        if ((rc = scr.get((size_t)batch * k * n, &sc1)))
+            return rc;
+        const long long total = batch * k * n;
+        B200_LAUNCH(galois_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, gal->in2, (u64 *)nullptr, sc1, ctx->logn, gal->g,
+                    total);
+        ctx->launches++;
+        d = sc1;
+        d_stride = (long long)k * n;
+    }
     if (!clustered)
     {
         std::vector<int> prime;
@@ -2040,7 +2109,12 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
     }
     {
         const long long total = batch * 2 * (n >> 1);
-        if (D)
+        if (gal)
+        {
+            DISPATCH_K(k, B200_LAUNCH(ksmoddown_galois_add_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special,
+                                      ctx->d_inv_qsp, ks2, gal->in2, gal->addend2, dst, ctx->logn, gal->ginv, total));
+        }
+        else if (D)
         {
             DISPATCH_K(k, B200_LAUNCH(scale_moddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, make_scale_fpc<KK>(ctx, level),
                                       ctx->d_primes, special, ctx->d_inv_qsp, D, ks2, dst, n, total));
@@ -2889,6 +2963,39 @@ int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t ga
     u64 *o = (u64 *)out2;
     return keyswitch_core(ctx, level, tmp, (long long)k * n, (const u64 *)galois_key, o, 2LL * k * n, nullptr, 0, o,
                           2LL * k * n, (long long)batch, s);
+}
+
+int b200_apply_galois_add(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
+                          const uint64_t *addend2, uint64_t *out2, uint64_t batch, void *stream)
+{
+    int rc = check_level(ctx, level);
+    if (rc)
+        return rc;
+    if (!in2 || !galois_key || !out2)
+        return fail(B200_E_NULL, "null pointer");
+    if (!(galois_elt & 1) || galois_elt >= 2 * ctx->n)
+        return fail(B200_E_INVALID, "Galois element is not valid");
+    const size_t bytes = (size_t)batch * 2 * ctx->levels[level].k * ctx->n * sizeof(u64);
+    auto overlap = [bytes](const void *a, const void *b) {
+        const char *x = (const char *)a, *y = (const char *)b;
+        return x < y + bytes && y < x + bytes;
+    };
+    if (batch && overlap(in2, out2))
+        return fail(B200_E_INVALID, "apply_galois_add: out overlaps in");
+    if (batch && addend2 && addend2 != out2 && overlap(addend2, out2))
+        return fail(B200_E_INVALID, "apply_galois_add: addend overlaps out without being out");
+    if (batch == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    // g^-1 mod 2n = g^(n-1): the odd residues mod 2n form a group of order n
+    const u64 m2 = 2 * (u64)ctx->n;
+    u64 ginv = 1, base = galois_elt;
+    for (u64 e = ctx->n - 1; e; e >>= 1, base = base * base % m2)
+        if (e & 1)
+            ginv = ginv * base % m2;
+    const KsGalois gal{ (const u64 *)in2, (const u64 *)addend2, galois_elt, (u32)ginv };
+    return keyswitch_core(ctx, level, nullptr, 0, (const u64 *)galois_key, nullptr, 0, nullptr, 0, (u64 *)out2, 0, (long long)batch,
+                          (cudaStream_t)stream, nullptr, &gal);
 }
 
 // plain [pb][n] -> out [pb][k][n]: each plaintext lifted to the level's residues and put in NTT form.  monomial != 0 gives

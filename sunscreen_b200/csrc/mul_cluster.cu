@@ -19,6 +19,7 @@
 // (the words of ks2, formed by the FP64 branch of ksmac_tma_kernel), so every word and every renorm bound equals the separate path's.
 #include "mul_cluster.h"
 #include "ntt_fp_body.cuh"
+#include <algorithm>
 #include <cuda_runtime.h>
 
 namespace
@@ -147,9 +148,12 @@ __device__ __forceinline__ KsPlace ks_place(int k)
 
 // The key switch's NTT-domain half for one (item, key residue I): forward transforms of the k digits mod p_I, inner product
 // with the key, inverse transforms of the two accumulators into ks2 [item][2][k + 1][n] (coefficient form, canonical).
-template <int LOGN>
-__global__ void __launch_bounds__(NT, 3) ks_cluster_kernel(const NttJob job, const u64 *d, long long d_stride, const u64 *key, int key_rows,
-                                                           u64 *ks2, int k)
+// GAL: the target is sigma_g(d) for the Galois element g with g^-1 mod 2n = ginv.  Digit J is gathered from d by the first
+// forward pass and negated mod q_J where the automorphism flips the sign, before its reduction mod p_I: the digits are the
+// integers the separate galois_kernel would have written, so every later word is unchanged.
+template <int LOGN, bool GAL>
+__device__ __forceinline__ void ks_cluster_body(const NttJob &job, const u64 *d, long long d_stride, const u64 *key, int key_rows,
+                                                u64 *ks2, int k, unsigned ginv)
 {
     extern __shared__ u64 mc_sm[];
     constexpr int N = 1 << LOGN;
@@ -160,7 +164,12 @@ __global__ void __launch_bounds__(NT, 3) ks_cluster_kernel(const NttJob job, con
         const NttPrimeFp PF = job.fprimes[job.slot_prime[w.I]];
         const NttPrime PI_ = job.primes[job.slot_prime[w.I]];
         // digit J of the target, reduced mod p_I by the first pass (job.reduce_input)
-        NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR>::run(job, PF, PI_, d + w.item * d_stride + (long long)w.J * N, nullptr, smd, tid, w.item, w.I);
+        const u64 *dj = d + w.item * d_stride + (long long)w.J * N;
+        if constexpr (GAL)
+            NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR | 8192>::run(job, PF, PI_, dj, nullptr, smd, tid, w.item, w.I, nullptr, ginv,
+                                                                    job.primes[job.slot_prime[w.J]].p);
+        else
+            NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR>::run(job, PF, PI_, dj, nullptr, smd, tid, w.item, w.I);
     }
     cluster_sync(); // all k digits transformed
     w = ks_place(k);
@@ -239,6 +248,20 @@ __global__ void __launch_bounds__(NT, 3) ks_cluster_kernel(const NttJob job, con
 }
 
 template <int LOGN>
+__global__ void __launch_bounds__(NT, 3) ks_cluster_kernel(const NttJob job, const u64 *d, long long d_stride, const u64 *key, int key_rows,
+                                                           u64 *ks2, int k)
+{
+    ks_cluster_body<LOGN, false>(job, d, d_stride, key, key_rows, ks2, k, 0);
+}
+
+template <int LOGN>
+__global__ void __launch_bounds__(NT, 3) ks_cluster_galois_kernel(const NttJob job, const u64 *d, long long d_stride, const u64 *key,
+                                                                  int key_rows, u64 *ks2, int k, unsigned ginv)
+{
+    ks_cluster_body<LOGN, true>(job, d, d_stride, key, key_rows, ks2, k, ginv);
+}
+
+template <int LOGN>
 cudaLaunchConfig_t config(long long clusters, cudaLaunchAttribute *at, cudaStream_t s, int csize = CLUSTER)
 {
     at[0].id = cudaLaunchAttributeClusterDimension;
@@ -302,14 +325,18 @@ int b200_ks_cluster_setup(int logn, int k, int *active)
     *active = 0;
     if (k < 2 || k > 8)
         return 0;
-    if (logn == 12)
-        return setup<12>(ks_cluster_kernel<12>, k, active);
-    if (logn == 13)
-        return setup<13>(ks_cluster_kernel<13>, k, active);
-    return 0;
+    // both variants: the same shared memory, and the register bound of __launch_bounds__; the smaller count of the two
+    int plain = 0, gal = 0, rc = 0;
+    if (logn == 12 && !(rc = setup<12>(ks_cluster_kernel<12>, k, &plain)))
+        rc = setup<12>(ks_cluster_galois_kernel<12>, k, &gal);
+    if (logn == 13 && !(rc = setup<13>(ks_cluster_kernel<13>, k, &plain)))
+        rc = setup<13>(ks_cluster_galois_kernel<13>, k, &gal);
+    *active = rc ? 0 : std::min(plain, gal);
+    return rc;
 }
 
-int b200_ks_cluster(int logn, const NttJob &job, const u64 *d, long long d_stride, const u64 *key, int key_rows, u64 *ks2, int k, void *stream)
+int b200_ks_cluster(int logn, const NttJob &job, const u64 *d, long long d_stride, const u64 *key, int key_rows, u64 *ks2, int k,
+                    unsigned galois_inv, void *stream)
 {
     cudaLaunchAttribute at[1];
     const long long clusters = job.items * (k + 1);
@@ -318,11 +345,15 @@ int b200_ks_cluster(int logn, const NttJob &job, const u64 *d, long long d_strid
     if (logn == 12)
     {
         const cudaLaunchConfig_t cfg = config<12>(clusters, at, (cudaStream_t)stream, k);
+        if (galois_inv)
+            return (int)cudaLaunchKernelEx(&cfg, ks_cluster_galois_kernel<12>, job, d, d_stride, key, key_rows, ks2, k, galois_inv);
         return (int)cudaLaunchKernelEx(&cfg, ks_cluster_kernel<12>, job, d, d_stride, key, key_rows, ks2, k);
     }
     if (logn == 13)
     {
         const cudaLaunchConfig_t cfg = config<13>(clusters, at, (cudaStream_t)stream, k);
+        if (galois_inv)
+            return (int)cudaLaunchKernelEx(&cfg, ks_cluster_galois_kernel<13>, job, d, d_stride, key, key_rows, ks2, k, galois_inv);
         return (int)cudaLaunchKernelEx(&cfg, ks_cluster_kernel<13>, job, d, d_stride, key, key_rows, ks2, k);
     }
     return (int)cudaErrorInvalidValue;

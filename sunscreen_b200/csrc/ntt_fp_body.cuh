@@ -468,12 +468,16 @@ template <int LOGN> struct NttSchedDone<LOGN, 0> { static constexpr int value = 
 // shared memory once per CTA and read from there (short latency, no L2 round trip per group); 2 / 4 / 8 = developer
 // ablations for tools/ntt_ablate.py (no twiddle loads / one-DMUL products / no global traffic): results are meaningless,
 // they only measure what each component costs.
+// VAR & 8192 (forward only): the first pass reads sigma_g(src) instead of src, for the Galois automorphism X -> X^g of a
+// coefficient-form row mod q: destination word e is source word i = e g^-1 mod 2n, negated mod q (gal_q) where i >= n.  `gal`
+// is g^-1 mod 2n.  The negation happens mod q, before job.reduce_input reduces the word mod the transform's prime.
 #define B200_NTT_TWS_ENTRIES 512
 template <int LOGN, int NT, bool FWD, int STEP /*0..NP-1 in execution order*/, int VAR = 0>
 struct NttFpStaticPass
 {
     static __device__ __forceinline__ void run(const NttJob &job, const NttPrimeFp &P, const NttPrime &PI_, const u64 *src, u64 *dst,
-                                               double *smd, int tid, long long item, int slot, const u64 *nsrc = nullptr)
+                                               double *smd, int tid, long long item, int slot, const u64 *nsrc = nullptr,
+                                               unsigned gal = 0, u64 gal_q = 0)
     {
 #if defined(__CUDA_ARCH__)
         constexpr int N = 1 << LOGN;
@@ -523,6 +527,13 @@ struct NttFpStaticPass
         constexpr bool KEEP_OUT = (VAR & 4096) != 0 && FWD, SMEM_IN = (VAR & 4096) != 0 && !FWD;
         constexpr bool SG = EDGE_IN && LOGS >= 5 && B200_NTT_DIRECT_IN && !STREAM && !SMEM_IN,
                        DG = EDGE_OUT && LOGS >= 5 && !(VAR & 128) && !KEEP_OUT; // 128: always stage the output
+        constexpr bool GATHER = (VAR & 8192) != 0 && FWD && EDGE_IN;
+        static_assert(!GATHER || SG, "the Galois gather reads the first pass's words straight from global memory");
+        auto gather_ld = [&](int e) -> u64 {
+            const unsigned i = ((unsigned)e * gal) & (2u * N - 1u);
+            const u64 x = src[i & (N - 1)];
+            return i < (unsigned)N ? x : (x ? gal_q - x : 0);
+        };
         constexpr bool TW16 = (L == 4 && LOGS == 0);
         constexpr int TWSRC = (VAR & 2) ? 2 : ((VAR & 1) && !TW16 && (1 << (DONE + L)) <= B200_NTT_TWS_ENTRIES) ? 1 : 0;
         constexpr int ABL = ((VAR & 4) ? 1 : 0) | ((VAR & (8 | 32)) ? 2 : 0) | ((VAR & (8 | 64)) ? 4 : 0) | ((VAR & 512) ? 8 : 0); // 32 / 64: loads / stores only; 512: streaming (evict-first) hints
@@ -666,7 +677,7 @@ struct NttFpStaticPass
                     }
                 }
             }
-            else if constexpr (SG && NGROUPS % NT == 0 && ITERS > 1)
+            else if constexpr (SG && NGROUPS % NT == 0 && ITERS > 1 && !GATHER)
             {
                 // direct first pass, software-pipelined: the raw words of group it+1 are requested before group `it` is
                 // transformed, so one DRAM latency is exposed per polynomial instead of one per group
@@ -696,6 +707,25 @@ struct NttFpStaticPass
 #pragma unroll
                     for (int j = 0; j < R; j++)
                         cur[j] = nxt[j];
+                }
+            }
+            else if constexpr (GATHER)
+            {
+                // the Galois gather: each group's words are loaded (scattered) right before it is transformed; no prefetch of
+                // the next group, whose registers the index arithmetic needs (the prefetching form spills)
+                constexpr int R = 1 << L;
+                static_assert(NGROUPS % NT == 0, "whole iterations");
+#pragma unroll
+                for (int it = 0; it < ITERS; it++)
+                {
+                    const int g = tid + it * NT, i0 = g >> LOGS, o0 = g & ((1 << LOGS) - 1);
+                    const int b0 = (i0 << (LOGS + L)) + o0;
+                    u64 cur[R];
+#pragma unroll
+                    for (int j = 0; j < R; j++)
+                        cur[j] = gather_ld(b0 + (j << LOGS));
+                    ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, true, false, false, TWSRC, ABL>(
+                        smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, cur, nullptr, stw);
                 }
             }
             else
@@ -832,7 +862,7 @@ struct NttFpStaticPass
             }
         }
         if (STEP + 1 < NP)
-            NttFpStaticPass<LOGN, NT, FWD, (STEP + 1 < NP ? STEP + 1 : STEP), VAR>::run(job, P, PI_, src, dst, smd, tid, item, slot, nsrc);
+            NttFpStaticPass<LOGN, NT, FWD, (STEP + 1 < NP ? STEP + 1 : STEP), VAR>::run(job, P, PI_, src, dst, smd, tid, item, slot, nsrc, gal, gal_q);
 #endif
     }
 };

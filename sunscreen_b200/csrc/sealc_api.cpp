@@ -2339,6 +2339,117 @@ long B200_Evaluator_MultiplyPlainSum(void *p, uint64_t rows, uint64_t cols, void
     });
 }
 
+// Rotate-and-sum slot reduction: destinations[i] receives the words of the chain
+//     c = encrypteds[i];  for s in steps: c = Add(c, RotateRows(c, s));  if columns: c = Add(c, RotateColumns(c))
+// A step whose key is present is one b200_apply_galois_add.  A step without its own key goes through its NAF parts as
+// op_rotate does (parts of +-n/2 skipped): the intermediate parts as b200_apply_galois, the last one fused with the add.  Step 0
+// adds c to itself.  Every step and key is checked before any work.  The items are gathered into one slab and the steps
+// ping-pong between two slabs, so destinations may alias encrypteds.  Only the final result is checked for transparency: a
+// transparent intermediate the chain would refuse is not detected (a transparent input, c1 = 0, stays transparent and is
+// reported).
+long B200_Evaluator_RotateSumBatch(void *p, uint64_t count, void **encs, int nsteps, const int *steps, bool columns,
+                                   void *galois_keys, void **dsts)
+{
+    NULLRET(p);
+    NULLRET(encs);
+    NULLRET(galois_keys);
+    NULLRET(dsts);
+    if (nsteps > 0)
+        NULLRET(steps);
+    auto *c = ((Evaluator_ *)p)->ctx;
+    auto &keys = *(KSwitchKeys_ *)galois_keys;
+    return guard([&] {
+        if (count == 0)
+            return;
+        if (!c->using_batching)
+            throw LogicErr("encryption parameters do not support batching");
+        if (nsteps < 0)
+            throw InvalidArg("nsteps must not be negative");
+        batch_handles(count, { encs, dsts });
+        if (keys.parms_id != c->ids[0])
+            throw InvalidArg("galois_keys is not valid for encryption parameters");
+        const size_t n = c->parms.n;
+        auto key_index = [&](uint32_t e) -> size_t {
+            const size_t idx = (e - 1) >> 1;
+            if (idx >= keys.keys.size() || keys.keys[idx].empty())
+                throw InvalidArg("Galois key not present");
+            check_keys(c, keys, idx);
+            return idx;
+        };
+        auto elt_of = [&](int st) {
+            uint32_t e = 0;
+            if (b200_galois_elt_from_step(c->dev, st, &e))
+                throw InvalidArg("step count too large");
+            return e;
+        };
+        // per step, the Galois elements the chain applies (empty: c + c)
+        std::vector<std::vector<uint32_t>> plan;
+        for (int i = 0; i < nsteps; i++)
+        {
+            std::vector<uint32_t> elts;
+            if (steps[i] != 0)
+            {
+                const uint32_t e = elt_of(steps[i]);
+                const size_t idx = (e - 1) >> 1;
+                if (idx < keys.keys.size() && !keys.keys[idx].empty())
+                    elts.push_back(e);
+                else
+                {
+                    const std::vector<int> parts = naf(steps[i]);
+                    if (parts.size() == 1)
+                        throw InvalidArg("Galois key not present");
+                    for (int st : parts)
+                        if ((size_t)std::abs(st) != (n >> 1))
+                            elts.push_back(elt_of(st));
+                }
+                for (uint32_t x : elts)
+                    key_index(x);
+            }
+            plan.push_back(std::move(elts));
+        }
+        if (columns)
+        {
+            key_index((uint32_t)(2 * n - 1));
+            plan.push_back({ (uint32_t)(2 * n - 1) });
+        }
+        OpScope scope(c);
+        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        const u64 w = batch_item_words(c, encs);
+        BatchSlab A(c, count * w), B(c, count * w);
+        std::unique_ptr<BatchSlab> T; // third slab for NAF steps of three or more parts
+        u64 k = 0;
+        const int lv = batch_gather(c, count, encs, A, k);
+        BatchSlab *cur = &A, *other = &B;
+        auto key = [&](uint32_t e) { return keys.flat_dev(c, key_index(e), (int)k); };
+        for (const auto &elts : plan)
+        {
+            if (elts.empty())
+            {
+                dev_check(b200_add(c->dev, lv, cur->w(), cur->w(), cur->w(), 2, count, cur_stream()));
+                continue;
+            }
+            if (elts.size() == 1)
+            {
+                dev_check(b200_apply_galois_add(c->dev, lv, cur->w(), elts[0], key(elts[0]), cur->w(), other->w(), count, cur_stream()));
+                std::swap(cur, other);
+                continue;
+            }
+            // NAF parts: the intermediates alternate between `other` and T; the last part adds into cur in place
+            if (elts.size() > 2 && !T)
+                T.reset(new BatchSlab(c, count * w));
+            const u64 *src = cur->w();
+            for (size_t j = 0; j + 1 < elts.size(); j++)
+            {
+                u64 *dst = src == other->w() ? T->w() : other->w();
+                dev_check(b200_apply_galois(c->dev, lv, src, elts[j], key(elts[j]), dst, count, cur_stream()));
+                src = dst;
+            }
+            dev_check(b200_apply_galois_add(c->dev, lv, src, elts.back(), key(elts.back()), cur->w(), cur->w(), count, cur_stream()));
+        }
+        batch_scatter(c, count, dsts, *cur, ((Ciphertext_ *)encs[0])->parms_id, k, lv);
+    });
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Decryptor
 // ---------------------------------------------------------------------------------------------------------

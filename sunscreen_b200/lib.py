@@ -74,6 +74,7 @@ _SIGS = {
     "b200_relinearize": [vp, C.c_int, vp, vp, vp, u64, vp],
     "b200_multiply_relin": [vp, C.c_int, vp, vp, vp, vp, u64, vp],
     "b200_apply_galois": [vp, C.c_int, vp, C.c_uint32, vp, vp, u64, vp],
+    "b200_apply_galois_add": [vp, C.c_int, vp, C.c_uint32, vp, vp, vp, u64, vp],
     "b200_multiply_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
     "b200_plain_to_ntt": [vp, C.c_int, vp, u64, vp, C.c_int, vp],
     "b200_multiply_plain_sum": [vp, C.c_int, vp, C.c_int, u64, vp, u64, vp, vp],
@@ -258,6 +259,11 @@ class B200Context:
     def apply_galois(self, in2, elt, key, out2, batch, level=None, stream=None):
         self.L.call("b200_apply_galois", self.h, self._lv(level), vp(ptr(in2)), C.c_uint32(elt), vp(ptr(key)), vp(ptr(out2)),
                     u64(batch), vp(stream))
+
+    def apply_galois_add(self, in2, elt, key, addend2, out2, batch, level=None, stream=None):
+        """out2 = addend2 + apply_galois(in2, elt) (addend2 None: no addend); addend2 may be in2 or out2, out2 must not overlap in2."""
+        self.L.call("b200_apply_galois_add", self.h, self._lv(level), vp(ptr(in2)), C.c_uint32(elt), vp(ptr(key)),
+                    vp(ptr(addend2)), vp(ptr(out2)), u64(batch), vp(stream))
 
     def multiply_plain(self, a, size, plain, plain_batch, out, batch, level=None, stream=None):
         self.L.call("b200_multiply_plain", self.h, self._lv(level), vp(ptr(a)), C.c_int(size), vp(ptr(plain)),
