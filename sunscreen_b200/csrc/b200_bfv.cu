@@ -3224,8 +3224,14 @@ int b200_mod_switch_to_next(b200_ctx *ctx, int level, const uint64_t *a, int siz
         return 0;
     const long long n = (long long)ctx->n;
     const long long total = (long long)batch * size * n;
-    DISPATCH_K(L.k, B200_LAUNCH(modswitch_kernel<KK>, blocks_for(total, EB), EB, 0, (cudaStream_t)stream, 
-                        ctx->d_primes, L.inv_qlast, (const u64 *)a, (u64 *)out, n, total));
+    // 17 residues: the key level of a chain with 16 data residues, which public-key encryption drops to its first data
+    // level.  modswitch_coeff is integer-only, so the FP64 bound that caps the other kernels at 16 does not apply.
+    if (L.k == 17)
+        B200_LAUNCH(modswitch_kernel<17>, blocks_for(total, EB), EB, 0, (cudaStream_t)stream, ctx->d_primes, L.inv_qlast,
+                    (const u64 *)a, (u64 *)out, n, total);
+    else
+        DISPATCH_K(L.k, B200_LAUNCH(modswitch_kernel<KK>, blocks_for(total, EB), EB, 0, (cudaStream_t)stream,
+                            ctx->d_primes, L.inv_qlast, (const u64 *)a, (u64 *)out, n, total));
     ctx->launches++;
     CU_TRY(cudaGetLastError());
     return 0;

@@ -91,6 +91,35 @@ PARAMS.update({
 SEC_NONE.add("n4096_9x22")
 LONG = list(LONG_BITS)
 
+# Wide chains (also from CoeffModulus::Create): n = 32768 beyond the default chain, and the key level of the longest chains.
+# Kept out of EDGE and LONG; tests/test_gpu_wide_chains.py runs them.
+WIDE_BITS = {
+    # 60-bit primes through the n = 32768 split transform (ntt_outer_kernel): the Harvey lazy bounds at their tightest
+    "n32768_60x6": (32768, [60] * 6),
+    # 30-bit primes under a 47-bit auxiliary base that needs fewer primes than k (nB < k), on the integer BEHZ kernels
+    # (the split transform switches the FP64 path off)
+    "n32768_30x5": (32768, [30] * 5),
+    # 60-bit digits reduced mod 30-bit primes (and back) in the split transform's input reduction, under the 61-bit base
+    "n32768_mixed": (32768, [60, 30, 30, 30, 60]),
+    # 16 data residues and 17 key-level primes at n = 32768 (833 bits <= 881), integer kernels against a 49-bit base
+    "n32768_49x17": (32768, [49] * 17),
+    # 17 data residues, one beyond the library's limit (432 bits <= 438): each op gives the reference's words or refuses
+    "n16384_24x18": (16384, [24] * 18),
+}
+PARAMS.update({
+    "n32768_60x6": (32768, [0xfffffffff330001, 0xfffffffff550001, 0xfffffffff5a0001, 0xfffffffff6a0001, 0xfffffffff840001,
+                            0xffffffffffc0001], 786433),
+    "n32768_30x5": (32768, [0x3fbb0001, 0x3fd20001, 0x3fde0001, 0x3fed0001, 0x3ffc0001], 786433),
+    "n32768_mixed": (32768, [0xfffffffff840001, 0x3fde0001, 0x3fed0001, 0x3ffc0001, 0xffffffffffc0001], 786433),
+    "n32768_49x17": (32768, [0x1ffffff0b0001, 0x1ffffff230001, 0x1ffffff330001, 0x1ffffff390001, 0x1ffffff510001,
+                             0x1ffffff570001, 0x1ffffff5c0001, 0x1ffffff780001, 0x1ffffff890001, 0x1ffffffa10001,
+                             0x1ffffffa20001, 0x1ffffffb00001, 0x1ffffffb40001, 0x1ffffffba0001, 0x1ffffffd40001,
+                             0x1ffffffea0001, 0x1fffffff50001], 786433),
+    "n16384_24x18": (16384, [0xbe0001, 0xbe8001, 0xc18001, 0xc78001, 0xca0001, 0xcb8001, 0xcf0001, 0xd00001, 0xd08001,
+                             0xd78001, 0xd80001, 0xe38001, 0xe40001, 0xee8001, 0xf60001, 0xfa0001, 0xfc0001, 0xfd0001], 786433),
+})
+WIDE = list(WIDE_BITS)
+
 # Plain moduli beyond 20 bits on chains above: name -> (chain, how t is chosen).  A batching t is what
 # PlainModulus::Batching(n, bits) returns, the largest prime = 1 mod 2n below 2^bits (CoeffModulus::Create(n, {bits})),
 # skipping the chain's own primes where noted; tests/test_params.py re-derives each.

@@ -240,12 +240,12 @@ def plain_operand_classes(n, t, rng):
     return [out[i] for i in rng.permutation(len(out))]
 
 
-def check_plain_operands(P, seed=41):
+def check_plain_operands(P, seed=41, levels=None):
     """multiply_plain / add_plain / sub_plain with every plaintext class of plain_operand_classes, one per item of a batch
-    (plain_batch == batch, so the monomial test is per item), at every data level of the reference's chain through
-    layer 1's `level` argument, word for word against the reference's Evaluator; then one monomial broadcast to every item
-    (plain_batch = 1).  Where the reference's product is transparent (a monomial t under a prime below t: Q - t + t = Q),
-    it refuses it and the layer-1 words must be all zero."""
+    (plain_batch == batch, so the monomial test is per item), at every data level of the reference's chain (or the data
+    levels `levels`, 0 = the first) through layer 1's `level` argument, word for word against the reference's Evaluator;
+    then one monomial broadcast to every item (plain_batch = 1).  Where the reference's product is transparent (a monomial
+    t under a prime below t: Q - t + t = Q), it refuses it and the layer-1 words must be all zero."""
     rng = np.random.default_rng(seed)
     R = P.ref
     classes = plain_operand_classes(P.n, P.t, rng)
@@ -258,7 +258,7 @@ def check_plain_operands(P, seed=41):
     minus_one[0, 0] = P.t - 1
     rpls = [R.new_pt(p) for p in plains]
     rp = R.new_pt(minus_one[0, :1])
-    for j in range(len(R.data_parms_ids())):
+    for j in range(len(R.data_parms_ids())) if levels is None else levels:
         lv = P.ctx.first_level + j
         k = P.ctx.level_info(lv)["k"]
         assert k == R.k - j
@@ -524,8 +524,9 @@ def _residues(X, q, n, rng):
     return np.array([[x % qi for x in X] for qi in q], dtype=np.uint64), X
 
 
-def check_decrypt(P, batch=5, seed=31):
-    """b200_ct_sk_phase and b200_decrypt at every data level of the reference's chain, with a real reference secret key
+def check_decrypt(P, batch=5, seed=31, levels=None):
+    """b200_ct_sk_phase and b200_decrypt at every data level of the reference's chain (or the data levels `levels`, 0 = the
+    first), with a real reference secret key
     (its NTT-form words; the powers s^2, s^3 come from Python integers):
     - uniformly random ciphertexts of size 2, 3 and 4, batch 5: the phase against independent_phase, the plaintext against
       the reference's Decryptor::decrypt (which accepts any ciphertext);
@@ -553,7 +554,7 @@ def check_decrypt(P, batch=5, seed=31):
         out[: got.size] = got
         return out
 
-    for j in range(len(R.data_parms_ids())):
+    for j in range(len(R.data_parms_ids())) if levels is None else levels:
         lv = P.ctx.first_level + j
         k = R.k - j
         assert P.ctx.level_info(lv)["k"] == k

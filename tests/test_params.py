@@ -6,7 +6,7 @@ import math
 
 import pytest
 
-from params import EDGE, EDGE_BITS, LONG, LONG_BITS, PARAMS, PLAIN_EDGE, PLAIN_EDGE_T, SEC_NONE
+from params import EDGE, EDGE_BITS, LONG, LONG_BITS, PARAMS, PLAIN_EDGE, PLAIN_EDGE_T, SEC_NONE, WIDE, WIDE_BITS
 
 
 def is_prime(v):
@@ -108,6 +108,45 @@ def test_long_chains_reach_their_cases():
     for name, widest in (("n16384_17x25", 25), ("n16384_49_16x24", 49)):
         n, m, t = PARAMS[name]
         assert len(m) - 1 == 16 and max(q.bit_length() for q in m) == widest
+
+
+@pytest.mark.parametrize("name", WIDE)
+def test_wide_chain_is_create_output(name):
+    n, bits = WIDE_BITS[name]
+    _, moduli, t = PARAMS[name]
+    assert [q.bit_length() for q in moduli] == bits
+    assert moduli == create_coeff_modulus(n, bits)
+    assert t == {16384: 786433, 32768: 786433}[n]                 # the default plain modulus of each n
+
+
+def test_wide_chains_reach_their_cases():
+    """What each wide chain is there for (host_ctx.h: FP64 primes are <= 49 bits, and the auxiliary base is then as wide as
+    the widest user prime, at least 47 bits, with enough primes that bits(prod(B) m_sk) > 32 + bits(t) + bits(Q); b200_bfv.cu:
+    the k-templated kernels take at most 16 data residues, modswitch_kernel 17 at the key level)."""
+    bits = lambda q: math.prod(q).bit_length()
+    widths = lambda name: {q.bit_length() for q in PARAMS[name][1]}
+    assert all(PARAMS[name][0] == 32768 for name in WIDE if name != "n16384_24x18")
+    assert widths("n32768_60x6") == {60}
+    assert widths("n32768_30x5") == {30}
+    n, m, t = PARAMS["n32768_mixed"]
+    assert [q.bit_length() for q in m] == [60, 30, 30, 30, 60] and m[0] < m[-1]        # the special prime is the widest
+    # n32768_30x5: k 47-bit primes (k - 1 in B, and m_sk) already cover the first data level's range, so nB < k (asserted on
+    # the library's own base by tests/test_gpu_wide_chains.py)
+    n, m, t = PARAMS["n32768_30x5"]
+    k = len(m) - 1
+    assert 46 * k > 33 + t.bit_length() + bits(m[:k])
+    # the 17-prime key levels: 16 data residues
+    for name in ("n16384_17x25", "n16384_49_16x24", "n32768_49x17"):
+        assert len(PARAMS[name][1]) == 17, name
+    assert widths("n32768_49x17") == {49}
+    # beyond the limit: 17 data residues, and still within 128-bit security at n = 16384 (438 bits)
+    n, m, t = PARAMS["n16384_24x18"]
+    assert len(m) - 1 == 17 and bits(m) <= 438 and sum(q.bit_length() for q in m) == 432
+
+
+@pytest.mark.parametrize("name", WIDE)
+def test_wide_chain_matches_reference_create(ref, name):
+    reference_create_matches(ref, name, *WIDE_BITS[name])
 
 
 def batching_plain_modulus(n, bits, skip=()):
