@@ -15,6 +15,7 @@
  *   b200_relinearize     Evaluator_Relinearize     S/c/evaluator.cpp:333      -> relinearize_internal     S/evaluator.cpp:1104-1159
  *   b200_apply_galois    Evaluator_ApplyGalois / RotateRows / RotateColumns   -> apply_galois_inplace     S/evaluator.cpp:2221-2323
  *   b200_apply_galois_add    apply_galois_inplace + add_inplace (one step of a rotate-and-sum reduction)
+ *   b200_multiply_relin_sum  a chain of multiply + relinearize + add_inplace (encrypted inner products)
  *   b200_add/sub/negate  Evaluator_Add/Sub/Negate                             -> S/evaluator.cpp:130-350
  *   b200_multiply_plain  Evaluator_MultiplyPlain                              -> multiply_plain_normal    S/evaluator.cpp:1858-1992
  *   b200_plain_to_ntt    Evaluator_TransformToNTT1                            -> transform_to_ntt_inplace S/evaluator.cpp:2033-2124
@@ -119,6 +120,11 @@ int b200_relinearize(b200_ctx *ctx, int level, const uint64_t *in3, const uint64
 /* multiply (2,2->3) followed by relinearize (3->2) without materialising the size-3 result in the caller's memory */
 int b200_multiply_relin(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, const uint64_t *relin_key,
                         uint64_t *out2, uint64_t batch, void *stream);
+/* out2[r] = sum_{j<m} relinearize(multiply(a[r][j], b[r][j])); a, b: [rows][m][2][k][n], out2: [rows][2][k][n].
+   b may equal a (squares).  out2 must not overlap a or b.  m == 0: B200_E_INVALID; rows == 0: no work.  The words of
+   b200_multiply_relin followed by m - 1 b200_add, with the adds folded into the key switch's mod-down. */
+int b200_multiply_relin_sum(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, const uint64_t *relin_key,
+                            uint64_t m, uint64_t *out2, uint64_t rows, void *stream);
 /* size-2 cts: out = (sigma_g(c0), 0) + KeySwitch(sigma_g(c1), galois_key) */
 int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
                       uint64_t *out2, uint64_t batch, void *stream);

@@ -298,6 +298,16 @@ SEAL_C_FUNC B200_Evaluator_MultiplyPlainSum(void *thisptr, uint64_t rows, uint64
    transparent input stays transparent).  All encrypteds at one level; destinations may alias encrypteds. */
 SEAL_C_FUNC B200_Evaluator_RotateSumBatch(void *thisptr, uint64_t count, void **encrypteds, int nsteps, const int *steps, bool columns,
                                           void *galois_keys, void **destinations);
+/* encrypted inner products: destinations[i] receives the words of
+       c = Relinearize(Multiply(encrypteds1[i*cols], encrypteds2[i*cols]));
+       for j = 1 ... cols-1: c = Add(c, Relinearize(Multiply(encrypteds1[i*cols + j], encrypteds2[i*cols + j])))
+   (both arrays row-major, rows x cols; the same handle twice in one term squares it).  Same checks and HRESULTs as that
+   chain, all made before any work, except: every operand must be a size-2 ciphertext (the chain's Relinearize refuses larger
+   products with single-key relinearization keys) at one level for the whole call, and a transparent intermediate is not
+   detected (only a term whose two operands are both transparent, and a transparent final result).  Destinations may alias
+   encrypteds. */
+SEAL_C_FUNC B200_Evaluator_MultiplyRelinSum(void *thisptr, uint64_t rows, uint64_t cols, void **encrypteds1, void **encrypteds2,
+                                            void *relin_keys, void **destinations);
 
 #ifdef __cplusplus
 }

@@ -547,6 +547,106 @@ __global__ void ksmoddown_galois_add_kernel(const PrimeDev *primes, int special_
     ksmoddown2<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, b, dst2 + off + c);
 }
 
+// ksmoddown2 with the result kept in registers: x[u][i] <- moddown(acc)_i + x[u][i] (mod q_i), x canonical.  The arithmetic is
+// ksmoddown2's word for word; only the store is replaced.
+template <int K>
+B200_DEV void ksmoddown2_regs(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *acc, long long n,
+                              u64 (&x)[2][K])
+{
+    const PrimeDev SP = ld_prime(&primes[special_idx]);
+    const u64 half = SP.p >> 1;
+    const b200_u64x2 sp = ldg2(acc + (long long)K * n);
+    u64 s0 = sp.x + half, s1 = sp.y + half;
+    s0 = s0 >= SP.p ? s0 - SP.p : s0;
+    s1 = s1 >= SP.p ? s1 - SP.p : s1;
+#pragma unroll
+    for (int i = 0; i < K; i++)
+    {
+        const PrimeDev Q = ld_prime(&primes[i]);
+        const u64 h = barrett64(half, Q.p, Q.r1);
+        const u64 w = B200_LDG(&inv_qsp[2 * i]), wq = B200_LDG(&inv_qsp[2 * i + 1]);
+        const b200_u64x2 a = ldg2(acc + (long long)i * n);
+        u64 v0 = a.x + (Q.p - barrett64(s0, Q.p, Q.r1)) + h;
+        u64 v1 = a.y + (Q.p - barrett64(s1, Q.p, Q.r1)) + h;
+        v0 = shoup_mul(v0, w, wq, Q.p);
+        v1 = shoup_mul(v1, w, wq, Q.p);
+        x[0][i] = add_mod(v0, x[0][i], Q.p);
+        x[1][i] = add_mod(v1, x[1][i], Q.p);
+    }
+}
+
+// b200_multiply_relin_sum's mod-down: out[u] = addend[u] + sum_{j < m} (base_j + moddown(ks2_j)) over the m items of output u,
+// in item order.  base_j = scale(D_j) where SCALE (FP64 levels that keep the products D, [item][3][K + |Bsk|][n] as
+// multiply_core's keep_D leaves them), else row `comp` of `base` ([item][2][K][n]: c0 / c1 scaled separately, or ciphertexts
+// to sum).  ks2 == nullptr: no key switch (a plain sum of the base items).  Canonical words summed mod q_i give one result for
+// any grouping, so the words are those of the multiply_relin + add chain.  Each output's items may be split into G groups of
+// consecutive items (group g of output r: items [g m / G, (g + 1) m / G) of r); dst is then [R][G][2][K][n], one partial sum
+// per group, and the addend ([R][2][K][n], nullptr: none) seeds group 0.  addend may be dst when G == 1 (each thread reads its
+// words before it writes them).  One thread per (output, group, component, two adjacent coefficients).
+template <int K, bool SCALE>
+__global__ void moddown_sum_kernel(const ScaleFpC<K> L, const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *D,
+                                   const u64 *base, const u64 *ks2, const u64 *addend, u64 *dst, int m, int G, long long n,
+                                   long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long hn = n >> 1;
+    const long long c = (idx % hn) * 2;
+    const long long t = idx / hn;
+    const int comp = (int)(t & 1);
+    const long long u = t >> 1;
+    const long long r = u / G;
+    const int g = (int)(u % G);
+    u64 acc[2][K];
+#pragma unroll
+    for (int i = 0; i < K; i++)
+    {
+        const b200_u64x2 v = (addend && g == 0) ? ldg2(addend + ((r * 2 + comp) * K + i) * n + c) : b200_u64x2{ 0, 0 };
+        acc[0][i] = v.x;
+        acc[1][i] = v.y;
+    }
+    const int j0 = (int)((long long)g * m / G), j1 = (int)((long long)(g + 1) * m / G);
+#pragma unroll 1
+    for (int j = j0; j < j1; j++)
+    {
+        const long long item = r * m + j;
+        if (SCALE)
+        {
+            u64 b[2][K];
+            scale2_fp<K>(L, D + ((item * 3 + comp) * (K + L.nBsk)) * n + c, n, b);
+#pragma unroll
+            for (int i = 0; i < K; i++)
+            {
+                const u64 p = __ldg(&primes[i].p);
+                acc[0][i] = add_mod(acc[0][i], b[0][i], p);
+                acc[1][i] = add_mod(acc[1][i], b[1][i], p);
+            }
+        }
+        else
+        {
+#pragma unroll
+            for (int i = 0; i < K; i++)
+            {
+                const u64 p = __ldg(&primes[i].p);
+                const b200_u64x2 v = ldg2(base + ((item * 2 + comp) * K + i) * n + c);
+                acc[0][i] = add_mod(acc[0][i], v.x, p);
+                acc[1][i] = add_mod(acc[1][i], v.y, p);
+            }
+        }
+        if (ks2)
+            ksmoddown2_regs<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, acc);
+    }
+    u64 *d = dst + (u * 2 + comp) * K * n + c;
+#pragma unroll
+    for (int i = 0; i < K; i++)
+        stg2(d + (long long)i * n, acc[0][i], acc[1][i]);
+}
+
+// the residue counts at which multiply_relin_sum keeps D for the scale inside moddown_sum_kernel (multiply_relin_one's rule
+// (k + 1)(k + 2) <= 4 (k + |Bsk|) in addition); above them c0 / c1 are scaled separately
+#define B200_MR_SUM_SCALE_MAX_K 8
+
 template <int K>
 __global__ void modswitch_kernel(const PrimeDev *primes, const u64 *inv_qlast, const u64 *src, u64 *dst, long long n,
                                  long long total)
@@ -1936,16 +2036,53 @@ struct KsGalois
     u32 g, ginv;              // the Galois element and its inverse mod 2n
 };
 
+// b200_multiply_relin_sum through keyswitch_core: the batch is R outputs of m consecutive items; dst[r] = addend[r] +
+// sum_j (base_j + moddown(ks2_j)) over the items of output r (moddown_sum_kernel)
+struct KsSum
+{
+    const u64 *base;   // [item][2][k][n] c0 / c1 of each product, or nullptr where D is kept (keyswitch_core's D)
+    const u64 *addend; // [R][2][k][n] or nullptr; may be dst
+    long long R;
+    int m;
+};
+
+// moddown_sum_kernel's term split: R outputs give R n / EB CTAs.  Where those would not fill the GPU (the kernel's resident
+// CTAs per SM times the SM count), the m terms of each output are split into G <= m groups, so that R G n / EB CTAs do; the
+// G partial sums then go through a second launch of the same kernel without a key switch.
+template <int K, bool SCALE>
+static int moddown_sum_groups(b200_ctx *ctx, long long R, int m)
+{
+    static int per_sm = 0; // one value per instantiation: the kernel's occupancy at EB threads per CTA
+    if (per_sm == 0)
+    {
+#ifdef B200_EMU_HEADER
+        per_sm = 2048 / EB;
+#else
+        int b = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, moddown_sum_kernel<K, SCALE>, EB, 0) != cudaSuccess || b < 1)
+            b = 1;
+        per_sm = b;
+#endif
+    }
+    const long long capacity = (long long)per_sm * ctx->sm_count;
+    const long long ctas = std::max<long long>(1, R * (long long)ctx->n / EB);
+    if (ctas >= capacity)
+        return 1;
+    return (int)std::min<long long>(m, (capacity + ctas - 1) / ctas);
+}
+
 // ---- key switch core: target d (k rows per item, stride d_stride), key list; dst_c = base_c + moddown(acc_c) ----
 // D (FP64 levels only; base0 / base1 unused): the unscaled products of multiply_core's keep_D; base_c = scale(D_c), formed in
 // the mod-down kernel; dst is then [item][2][k][n]
 // gal (d, d_stride, base0 / base1 unused): the rotate-add of KsGalois.  The cluster kernel gathers sigma_g(c1) in its digit loads;
 // otherwise galois_kernel writes sigma_g(c1) alone to scratch for the separate kernels.  The mod-down gathers sigma_g(c0) and adds
 // the addend (ksmoddown_galois_add_kernel); dst is then [item][2][k][n]
+// sum (base0 / base1 unused): the multiply_relin sums of KsSum (moddown_sum_kernel, with D where given); dst is then
+// [sum->R][2][k][n]
 static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_stride, const u64 *key, const u64 *base0,
                           long long base0_stride, const u64 *base1, long long base1_stride, u64 *dst,
                           long long dst_stride, long long batch, cudaStream_t s, const u64 *D = nullptr,
-                          const KsGalois *gal = nullptr)
+                          const KsGalois *gal = nullptr, const KsSum *sum = nullptr)
 {
     if (!ctx->host->using_keyswitching || level < 1)
         return fail(B200_E_LOGIC, "keyswitching is not supported by the context");
@@ -2107,6 +2244,56 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         if ((rc = launch_ntt<false>(ctx, jd, ks2, 2LL * (k + 1) * n, ks2, 2LL * (k + 1) * n, batch, 0, s)))
             return rc;
     }
+    if (sum)
+    {
+        // the SCALE variant exists up to B200_MR_SUM_SCALE_MAX_K residues (multiply_relin_sum_one keeps D only there)
+        int G = 1;
+        const long long R = sum->R;
+        u64 *part = nullptr;
+        auto launch = [&](auto kk, auto scale) -> int {
+            constexpr int KK = decltype(kk)::value;
+            constexpr bool SC = decltype(scale)::value && KK <= B200_MR_SUM_SCALE_MAX_K;
+            G = moddown_sum_groups<KK, SC>(ctx, R, sum->m);
+            int rc2;
+            if (G > 1 && (rc2 = scr.get((size_t)R * G * 2 * k * n, &part)))
+                return rc2;
+            const long long total = R * G * 2 * (n >> 1);
+            void (*k1)(const ScaleFpC<KK>, const PrimeDev *, int, const u64 *, const u64 *, const u64 *, const u64 *, const u64 *, u64 *,
+                       int, int, long long, long long) = moddown_sum_kernel<KK, SC>;
+#ifndef B200_EMU_HEADER
+            if (trace_on())
+                g_trace_name = "moddown_sum_kernel";
+#endif
+            B200_LAUNCH(k1, blocks_for(total, EB), EB, 0, s, SC ? make_scale_fpc<KK>(ctx, level) : ScaleFpC<KK>{}, ctx->d_primes,
+                        special, ctx->d_inv_qsp, D, sum->base, ks2, G > 1 ? nullptr : sum->addend, G > 1 ? part : dst, sum->m, G, n, total);
+            ctx->launches++;
+            if (G > 1)
+            {
+                // the G partial sums of each output, without a key switch
+                const long long total2 = R * 2 * (n >> 1);
+                k1 = moddown_sum_kernel<KK, false>;
+#ifndef B200_EMU_HEADER
+                if (trace_on())
+                    g_trace_name = "moddown_sum_kernel";
+#endif
+                B200_LAUNCH(k1, blocks_for(total2, EB), EB, 0, s, ScaleFpC<KK>{}, ctx->d_primes, special, ctx->d_inv_qsp,
+                            (const u64 *)nullptr, (const u64 *)part, (const u64 *)nullptr, sum->addend, dst, G, 1, n, total2);
+                ctx->launches++;
+            }
+            return 0;
+        };
+        if (D && k > B200_MR_SUM_SCALE_MAX_K)
+            return fail(B200_E_INVALID, "moddown_sum_kernel: no scaling variant at this residue count");
+        if (D)
+        {
+            DISPATCH_K(k, if ((rc = launch(std::integral_constant<int, KK>(), std::true_type()))) return rc);
+        }
+        else
+        {
+            DISPATCH_K(k, if ((rc = launch(std::integral_constant<int, KK>(), std::false_type()))) return rc);
+        }
+    }
+    else
     {
         const long long total = batch * 2 * (n >> 1);
         if (gal)
@@ -2930,6 +3117,100 @@ int b200_multiply_relin(b200_ctx *ctx, int level, const uint64_t *a, const uint6
         CU_TRY(cudaEventRecord(ctx->ev_join[p], ctx->s_side[p]));
         CU_TRY(cudaStreamWaitEvent(us, ctx->ev_join[p], 0));
     }
+    return rc;
+}
+
+// out[r] = addend[r] + sum_{j < m} relinearize(multiply(a[r][j], b[r][j])) for r < rows: multiply_relin_one over the rows m
+// items with keyswitch_core's sum mod-down (moddown_sum_kernel) in place of the per-item one.  D is kept on multiply_relin_one's
+// rule; otherwise c0 / c1 of every product go to scratch ([item][2][k][n]) and the mod-down sums them from there.
+static int multiply_relin_sum_one(b200_ctx *ctx, int level, const u64 *a, const u64 *b, const u64 *relin_key, int m, u64 *out2,
+                                  long long rows, const u64 *addend, cudaStream_t s)
+{
+    const long long n = (long long)ctx->n;
+    const LevelDev &L = ctx->levels[level];
+    const int k = L.k, R = k + L.nBsk;
+    const long long items = rows * m;
+    Scratch scr(ctx, s);
+    u64 *c2 = nullptr, *D = nullptr, *c01 = nullptr;
+    int rc;
+    if ((rc = scr.get((size_t)items * k * n, &c2)))
+        return rc;
+    if (L.fp && (k + 1) * (k + 2) <= 4 * R && k <= B200_MR_SUM_SCALE_MAX_K)
+    {
+        const KsSum sum{ nullptr, addend, rows, m };
+        if ((rc = scr.get((size_t)items * 3 * R * n, &D)))
+            return rc;
+        if ((rc = multiply_core(ctx, level, a, 2, b, 2, false, nullptr, 2, c2, items, s, D)))
+            return rc;
+        return keyswitch_core(ctx, level, c2, (long long)k * n, relin_key, nullptr, 0, nullptr, 0, out2, 0, items, s, D, nullptr, &sum);
+    }
+    if ((rc = scr.get((size_t)items * 2 * k * n, &c01)))
+        return rc;
+    if ((rc = multiply_core(ctx, level, a, 2, b, 2, false, c01, 2, c2, items, s)))
+        return rc;
+    const KsSum sum{ c01, addend, rows, m };
+    return keyswitch_core(ctx, level, c2, (long long)k * n, relin_key, nullptr, 0, nullptr, 0, out2, 0, items, s, nullptr, nullptr, &sum);
+}
+
+int b200_multiply_relin_sum(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, const uint64_t *relin_key, uint64_t m,
+                            uint64_t *out2, uint64_t rows, void *stream)
+{
+    int rc = check_level(ctx, level);
+    if (rc)
+        return rc;
+    if (!a || !b || !relin_key || !out2)
+        return fail(B200_E_NULL, "null pointer");
+    if (m == 0)
+        return fail(B200_E_INVALID, "a sum needs at least one term");
+    if (m > 0x7fffffffULL)
+        return fail(B200_E_INVALID, "too many terms");
+    if (rows == 0)
+        return 0;
+    if (!ctx->host->using_keyswitching || level < 1)
+        return fail(B200_E_LOGIC, "keyswitching is not supported by the context");
+    const long long n = (long long)ctx->n;
+    const LevelDev &L = ctx->levels[level];
+    const int k = L.k, R = k + L.nBsk;
+    const size_t w = (size_t)2 * k * n; // words of one ciphertext
+    {
+        const uintptr_t o0 = (uintptr_t)out2, o1 = o0 + rows * w * sizeof(u64);
+        const uintptr_t span = rows * m * w * sizeof(u64);
+        for (const uint64_t *x : { a, b })
+            if ((uintptr_t)x < o1 && o0 < (uintptr_t)x + span)
+                return fail(B200_E_INVALID, "multiply_relin_sum: out overlaps an operand");
+    }
+    CU_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    // scratch of one term at its peak: c2 with D (or c0 / c1) held, plus the larger of the multiply's ext + D and the key
+    // switch's ks1 + ks2
+    const bool keepD = L.fp && (k + 1) * (k + 2) <= 4 * R && k <= B200_MR_SUM_SCALE_MAX_K;
+    const size_t held = (size_t)k + (keepD ? 3 * R : 2 * k);
+    const size_t term_bytes = (held + std::max<size_t>((size_t)7 * R, (size_t)(k + 1) * (k + 2))) * n * sizeof(u64);
+    uint64_t cap = 1ull << 30;
+    if (const char *e = std::getenv("B200_MR_SUM_SCRATCH"))
+        cap = std::min<uint64_t>(cap, std::max<uint64_t>(1, strtoull(e, nullptr, 10)));
+    const uint64_t terms = std::max<uint64_t>(1, cap / term_bytes); // terms per launch sequence
+    const u64 *A = (const u64 *)a, *B = (const u64 *)b, *K = (const u64 *)relin_key;
+    u64 *O = (u64 *)out2;
+    if (m <= terms)
+    {
+        // chunks of whole outputs
+        const uint64_t per = std::max<uint64_t>(1, terms / m);
+        for (uint64_t r0 = 0; r0 < rows && !rc; r0 += per)
+        {
+            const uint64_t r = std::min(per, rows - r0);
+            rc = multiply_relin_sum_one(ctx, level, A + r0 * m * w, B + r0 * m * w, K, (int)m, O + r0 * w, (long long)r, nullptr, s);
+        }
+        return rc;
+    }
+    // one output at a time, its terms in chunks, the partial sum carried in out as the next chunk's addend
+    for (uint64_t r0 = 0; r0 < rows && !rc; r0++)
+        for (uint64_t j0 = 0; j0 < m && !rc; j0 += terms)
+        {
+            const uint64_t c = std::min(terms, m - j0);
+            rc = multiply_relin_sum_one(ctx, level, A + (r0 * m + j0) * w, B + (r0 * m + j0) * w, K, (int)c, O + r0 * w, 1,
+                                        j0 ? O + r0 * w : nullptr, s);
+        }
     return rc;
 }
 

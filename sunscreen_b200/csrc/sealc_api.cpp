@@ -2339,6 +2339,98 @@ long B200_Evaluator_MultiplyPlainSum(void *p, uint64_t rows, uint64_t cols, void
     });
 }
 
+// Encrypted inner products: destinations[i] receives the words of the chain
+//     c = Relinearize(Multiply(e1[i cols], e2[i cols]));  c = Add(c, Relinearize(Multiply(e1[i cols + j], e2[i cols + j]))), j >= 1
+// as one b200_multiply_relin_sum over the gathered operands.  Every term is checked in chain order before any work: Multiply's
+// metadata, level and NTT-form checks, then Relinearize's key and size checks.  A term whose operands are both transparent
+// (the chain's Multiply result is transparent) is found on the gathered slabs before the sum runs.  A transparent partial sum
+// is not detected, only a transparent final result.  Operands are gathered before the first scatter, so destinations may
+// alias them.
+long B200_Evaluator_MultiplyRelinSum(void *p, uint64_t rows, uint64_t cols, void **e1, void **e2, void *relin_keys, void **dsts)
+{
+    NULLRET(p);
+    NULLRET(e1);
+    NULLRET(e2);
+    NULLRET(relin_keys);
+    NULLRET(dsts);
+    if (rows == 0)
+        return 0;
+    if (cols == 0)
+        return E_INVALIDARG_;
+    const uint64_t terms = rows * cols;
+    for (uint64_t i = 0; i < terms; i++)
+    {
+        NULLRET(e1[i]);
+        NULLRET(e2[i]);
+    }
+    for (uint64_t i = 0; i < rows; i++)
+        NULLRET(dsts[i]);
+    auto *c = ((Evaluator_ *)p)->ctx;
+    auto &keys = *(KSwitchKeys_ *)relin_keys;
+    return guard([&] {
+        const int lv = data_level(c, *(Ciphertext_ *)e1[0], "encrypted1 is not valid for encryption parameters");
+        bool same = true; // every term a square of one handle: one gathered slab serves both operands
+        for (uint64_t t = 0; t < terms; t++)
+        {
+            auto &a = *(Ciphertext_ *)e1[t];
+            auto &b = *(Ciphertext_ *)e2[t];
+            // Multiply
+            const int la = data_level(c, a, "encrypted1 is not valid for encryption parameters");
+            data_level(c, b, "encrypted2 is not valid for encryption parameters");
+            if (a.parms_id != b.parms_id || la != lv)
+                throw InvalidArg("encrypted1 and encrypted2 parameter mismatch");
+            if (a.is_ntt_form || b.is_ntt_form)
+                throw InvalidArg("encrypted1 or encrypted2 cannot be in NTT form");
+            if (a.size + b.size - 1 > 16)
+                throw InvalidArg("invalid size");
+            // Relinearize of the size a.size + b.size - 1 product
+            if (keys.parms_id != c->ids[0])
+                throw InvalidArg("relin_keys is not valid for encryption parameters");
+            if (a.size != 2 || b.size != 2 || keys.keys.empty())
+                throw InvalidArg("not enough relinearization keys");
+            check_keys(c, keys, 0);
+            if (keys.keys[0].size() < (size_t)a.k)
+                throw InvalidArg("kswitch_keys is not valid for encryption parameters");
+            same = same && e1[t] == e2[t];
+        }
+        OpScope scope(c);
+        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        const u64 w = batch_item_words(c, e1);
+        BatchSlab A(c, terms * w);
+        std::unique_ptr<BatchSlab> B;
+        u64 k = 0, kb = 0;
+        batch_gather(c, terms, e1, A, k);
+        if (!same)
+        {
+            B.reset(new BatchSlab(c, terms * w));
+            batch_gather(c, terms, e2, *B, kb);
+        }
+        const u64 *pb = same ? A.w() : B->w();
+        if (c->check_transparent)
+        { // the chain's Multiply refuses a product of two transparent operands
+            BatchSlab flags(c, (terms + 1) / 2);
+            std::vector<uint32_t> fa(terms), fb(terms);
+            dev_check(b200_is_transparent(c->dev, lv, A.w(), 2, (uint32_t *)flags.p, terms, cur_stream()));
+            dev_check(b200_memcpy_d2h(c->dev, fa.data(), flags.p, terms * 4, cur_stream()));
+            scope.wait();
+            if (same)
+                fb = fa;
+            else
+            {
+                dev_check(b200_is_transparent(c->dev, lv, pb, 2, (uint32_t *)flags.p, terms, cur_stream()));
+                dev_check(b200_memcpy_d2h(c->dev, fb.data(), flags.p, terms * 4, cur_stream()));
+                scope.wait();
+            }
+            for (uint64_t t = 0; t < terms; t++)
+                if (fa[t] && fb[t])
+                    throw LogicErr("result ciphertext is transparent");
+        }
+        BatchSlab O(c, rows * w);
+        dev_check(b200_multiply_relin_sum(c->dev, lv, A.w(), pb, keys.flat_dev(c, 0, (int)k), cols, O.w(), rows, cur_stream()));
+        batch_scatter(c, rows, dsts, O, ((Ciphertext_ *)e1[0])->parms_id, k, lv);
+    });
+}
+
 // Rotate-and-sum slot reduction: destinations[i] receives the words of the chain
 //     c = encrypteds[i];  for s in steps: c = Add(c, RotateRows(c, s));  if columns: c = Add(c, RotateColumns(c))
 // A step whose key is present is one b200_apply_galois_add.  A step without its own key goes through its NAF parts as

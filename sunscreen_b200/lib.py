@@ -75,6 +75,7 @@ _SIGS = {
     "b200_multiply_relin": [vp, C.c_int, vp, vp, vp, vp, u64, vp],
     "b200_apply_galois": [vp, C.c_int, vp, C.c_uint32, vp, vp, u64, vp],
     "b200_apply_galois_add": [vp, C.c_int, vp, C.c_uint32, vp, vp, vp, u64, vp],
+    "b200_multiply_relin_sum": [vp, C.c_int, vp, vp, vp, u64, vp, u64, vp],
     "b200_multiply_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
     "b200_plain_to_ntt": [vp, C.c_int, vp, u64, vp, C.c_int, vp],
     "b200_multiply_plain_sum": [vp, C.c_int, vp, C.c_int, u64, vp, u64, vp, vp],
@@ -255,6 +256,12 @@ class B200Context:
     def multiply_relin(self, a, b, rlk, out2, batch, level=None, stream=None):
         self.L.call("b200_multiply_relin", self.h, self._lv(level), vp(ptr(a)), vp(ptr(b)), vp(ptr(rlk)), vp(ptr(out2)),
                     u64(batch), vp(stream))
+
+    def multiply_relin_sum(self, a, b, rlk, m, out2, rows, level=None, stream=None):
+        """out2[r] = sum_j relinearize(multiply(a[r][j], b[r][j])): a, b [rows][m][2][k][n] (b may be a: squares), out2
+        [rows][2][k][n], which must not overlap a or b."""
+        self.L.call("b200_multiply_relin_sum", self.h, self._lv(level), vp(ptr(a)), vp(ptr(b)), vp(ptr(rlk)), u64(m),
+                    vp(ptr(out2)), u64(rows), vp(stream))
 
     def apply_galois(self, in2, elt, key, out2, batch, level=None, stream=None):
         self.L.call("b200_apply_galois", self.h, self._lv(level), vp(ptr(in2)), C.c_uint32(elt), vp(ptr(key)), vp(ptr(out2)),
