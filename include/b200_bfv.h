@@ -20,6 +20,8 @@
  *   b200_multiply_plain  Evaluator_MultiplyPlain                              -> multiply_plain_normal    S/evaluator.cpp:1858-1992
  *   b200_plain_to_ntt    Evaluator_TransformToNTT1                            -> transform_to_ntt_inplace S/evaluator.cpp:2033-2124
  *   b200_multiply_plain_sum  a chain of multiply_plain + add_inplace (plaintext matrix x ciphertext vector)
+ *   b200_apply_galois_many   apply_galois_inplace over items with their own element and key, one key switch
+ *   b200_linear_transform    the baby-step giant-step chain of rotate_rows + multiply_plain + add_inplace (slot-wise matrix)
  *   b200_add_plain / b200_sub_plain   Evaluator_AddPlain/SubPlain             -> S/util/scalingvariant.cpp:69-188
  *   b200_mod_switch_to_next           Evaluator_ModSwitchToNext1              -> S/util/rns.cpp:801-840
  *   b200_ntt_forward / b200_ntt_inverse  (util level)                         -> S/util/ntt.cpp:393-474
@@ -134,6 +136,12 @@ int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t ga
    rotate-and-sum slot reduction (c = c + rotate_rows(c, s)). */
 int b200_apply_galois_add(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
                           const uint64_t *addend2, uint64_t *out2, uint64_t batch, void *stream);
+/* out2[i] = apply_galois(in2[src_idx ? src_idx[i] : i], elts[i]) with key list keys[i], word for word, as one key switch whose
+   items carry their own element and key.  src_idx, elts and keys are HOST arrays of `batch` entries; keys[i] are device key
+   lists as b200_apply_galois takes them.  Items with one key should be adjacent: below the key switch's cluster rule the
+   MAC runs once per run of equal keys.  out2 must not overlap the sources in2[0 .. max src_idx]. */
+int b200_apply_galois_many(b200_ctx *ctx, int level, const uint64_t *in2, const uint64_t *src_idx, const uint32_t *elts,
+                           const uint64_t *const *keys, uint64_t *out2, uint64_t batch, void *stream);
 /* plain: [batch or 1][n] coefficients mod t (plain_batch = 1 broadcasts one plaintext to every item).  multiply_plain
    follows the reference per plaintext item: an item with exactly one nonzero coefficient m is multiplied by m itself
    (its monomial path); any other item, and a monomial item when some q_i <= t, by the lifted plaintext
@@ -153,6 +161,15 @@ int b200_plain_to_ntt(b200_ctx *ctx, int level, const uint64_t *plain, uint64_t 
    overlap cts.  Each ciphertext is transformed once and each output once; m or R = 0 is a no-op. */
 int b200_multiply_plain_sum(b200_ctx *ctx, int level, const uint64_t *cts, int size, uint64_t m, const uint64_t *plain_ntt,
                             uint64_t R, uint64_t *out, void *stream);
+/* Baby-step giant-step slot-wise linear transform of V ciphertexts, word for word the chain
+       inner_g = sum_{j < baby} multiply_plain(apply_galois(ct, elts[j - 1]), P[g][j])    (j = 0: ct itself)
+       out     = inner_0 + sum_{1 <= g < giant} apply_galois(inner_g, elts[baby - 1 + g - 1])   (add, in order of g)
+   cts, out: [V][2][k][n] coefficient form (out may be cts, or must not overlap it).  elts, keys: HOST arrays of the baby - 1
+   baby-step then giant - 1 giant-step elements and device key lists.  plain_ntt: [giant][baby][k][n] from b200_plain_to_ntt
+   (B200_PLAIN_NTT_MULTIPLY).  present: HOST [giant][baby] mask of terms, or NULL for all; an absent term is skipped, a step no
+   present term uses needs no element or key, and a row without a present term is dropped.  No present term: an error. */
+int b200_linear_transform(b200_ctx *ctx, int level, const uint64_t *cts, uint64_t V, int baby, int giant, const uint32_t *elts,
+                          const uint64_t *const *keys, const uint64_t *plain_ntt, const uint8_t *present, uint64_t *out, void *stream);
 int b200_add_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t plain_batch,
                    uint64_t *out, uint64_t batch, void *stream);
 int b200_sub_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, const uint64_t *plain, uint64_t plain_batch,

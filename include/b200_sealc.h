@@ -308,6 +308,22 @@ SEAL_C_FUNC B200_Evaluator_RotateSumBatch(void *thisptr, uint64_t count, void **
    encrypteds. */
 SEAL_C_FUNC B200_Evaluator_MultiplyRelinSum(void *thisptr, uint64_t rows, uint64_t cols, void **encrypteds1, void **encrypteds2,
                                             void *relin_keys, void **destinations);
+/* row rotations by a step per item: destinations[i] receives the words of Evaluator_RotateRows(encrypteds[i], steps[i]), with
+   one key switch for the whole batch.  Same checks and HRESULTs as those calls, all made before any work, except: a step
+   without its own Galois key is E_INVALIDARG (RotateRows would split it into NAF parts), and all encrypteds are at one level.
+   Destinations may alias encrypteds. */
+SEAL_C_FUNC B200_Evaluator_RotateRowsStepsBatch(void *thisptr, uint64_t count, void **encrypteds, const int *steps, void *galois_keys,
+                                                void **destinations);
+/* baby-step giant-step slot-wise linear transform: destinations[i] receives the words of
+       inner_g = Add over j of MultiplyPlain(RotateRows(encrypteds[i], j), plains[g*baby + j])   (j = 0: encrypteds[i] itself)
+       c = inner_0;  for g = 1 ... giant-1: c = Add(c, RotateRows(inner_g, g*baby))
+   plains: giant x baby coefficient-form plaintexts (BatchEncoder output), row-major; a NULL handle is an absent term (skipped;
+   a row without terms is dropped).  Same checks and HRESULTs as that chain, all made before any work, except: a step without
+   its own Galois key is E_INVALIDARG (create the keys with KeyGenerator_CreateGaloisKeysFromSteps for steps 1 ... baby-1 and
+   g*baby), all encrypteds are at one level, and a transparent partial sum is not detected (only a transparent final result).
+   baby or giant 0 and a call where every term is absent are E_INVALIDARG.  Destinations may alias encrypteds. */
+SEAL_C_FUNC B200_Evaluator_LinearTransform(void *thisptr, uint64_t count, void **encrypteds, uint64_t baby, uint64_t giant, void **plains,
+                                           void *galois_keys, void **destinations);
 
 #ifdef __cplusplus
 }

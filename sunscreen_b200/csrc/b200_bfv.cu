@@ -643,6 +643,88 @@ __global__ void moddown_sum_kernel(const ScaleFpC<K> L, const PrimeDev *primes, 
         stg2(d + (long long)i * n, acc[0][i], acc[1][i]);
 }
 
+// sigma_g(c0) of a [2][K][n] ciphertext at the two adjacent destination coefficients c, c + 1, added to b[0][i] / b[1][i]
+// (ksmoddown_galois_add_kernel's gather: source i = c g^-1 mod 2n, negated mod q_i where i >= n)
+template <int K>
+B200_DEV void add_galois_c0(const PrimeDev *primes, const u64 *ct, int logn, u32 ginv, long long c, u64 (&b)[2][K])
+{
+    const long long n = 1LL << logn;
+    const u64 m2 = 2 * (u64)n - 1, i0 = ((u64)c * ginv) & m2, i1 = ((u64)(c + 1) * ginv) & m2;
+#pragma unroll
+    for (int i = 0; i < K; i++)
+    {
+        const u64 p = __ldg(&primes[i].p);
+        const u64 *row = ct + (long long)i * n;
+        const u64 s0 = __ldg(row + (i0 & (n - 1))), s1 = __ldg(row + (i1 & (n - 1)));
+        b[0][i] = add_mod(b[0][i], (i0 >> logn) ? neg_mod(s0, p) : s0, p);
+        b[1][i] = add_mod(b[1][i], (i1 >> logn) ? neg_mod(s1, p) : s1, p);
+    }
+}
+
+// b200_apply_galois_many's mod-down: ksmoddown_galois_add_kernel without an addend, item i gathering sigma_{g_i}(c0) from
+// tab[i].ct and writing tab[i].dst ([2][K][n]).  One thread per (item, component, two adjacent coefficients).
+template <int K>
+__global__ void ksmoddown_galois_many_kernel(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *ks2,
+                                             const B200GalItem *tab, int logn, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long n = 1LL << logn;
+    const long long hn = n >> 1;
+    const long long c = (idx % hn) * 2;
+    const long long t = idx / hn;
+    const int comp = (int)(t & 1);
+    const long long item = t >> 1;
+    u64 b[2][K];
+#pragma unroll
+    for (int i = 0; i < K; i++)
+        b[0][i] = b[1][i] = 0;
+    if (comp == 0)
+        add_galois_c0<K>(primes, tab[item].ct, logn, tab[item].ginv, c, b);
+    ksmoddown2<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, b, tab[item].dst + comp * K * n + c);
+}
+
+// The giant steps of the BSGS linear transform: dst[r] = addend[r] + sum_{j < m} apply_galois(tab[j R + r].ct, g_{j R + r}),
+// each term sigma_g(c0) + moddown(ks2), summed in registers in term order as moddown_sum_kernel does.  Canonical words summed
+// mod q_i give one result for any grouping, so the words are those of the rotate + add chain.  addend [R][2][K][n] (nullptr:
+// zero) may be dst.  One thread per (output, component, two adjacent coefficients).
+template <int K>
+__global__ void moddown_galois_sum_kernel(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *ks2,
+                                          const B200GalItem *tab, const u64 *addend, u64 *dst, int m, long long R, int logn,
+                                          long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long n = 1LL << logn;
+    const long long hn = n >> 1;
+    const long long c = (idx % hn) * 2;
+    const long long t = idx / hn;
+    const int comp = (int)(t & 1);
+    const long long r = t >> 1;
+    u64 acc[2][K];
+#pragma unroll
+    for (int i = 0; i < K; i++)
+    {
+        const b200_u64x2 v = addend ? ldg2(addend + ((r * 2 + comp) * K + i) * n + c) : b200_u64x2{ 0, 0 };
+        acc[0][i] = v.x;
+        acc[1][i] = v.y;
+    }
+#pragma unroll 1
+    for (int j = 0; j < m; j++)
+    {
+        const long long item = (long long)j * R + r;
+        if (comp == 0)
+            add_galois_c0<K>(primes, tab[item].ct, logn, tab[item].ginv, c, acc);
+        ksmoddown2_regs<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, acc);
+    }
+    u64 *d = dst + (r * 2 + comp) * K * n + c;
+#pragma unroll
+    for (int i = 0; i < K; i++)
+        stg2(d + (long long)i * n, acc[0][i], acc[1][i]);
+}
+
 // the residue counts at which multiply_relin_sum keeps D for the scale inside moddown_sum_kernel (multiply_relin_one's rule
 // (k + 1)(k + 2) <= 4 (k + |Bsk|) in addition); above them c0 / c1 are scaled separately
 #define B200_MR_SUM_SCALE_MAX_K 8
@@ -678,6 +760,22 @@ __global__ void galois_kernel(const PrimeDev *primes, int k, const u64 *in2, u64
     const u64 *src = in2 + ((item * 2 + poly) * k + r) * n;
     u64 *dst = poly == 0 ? out2 + ((item * 2) * k + r) * n : tmp + (item * k + r) * n;
     galois_coeff(p, src, dst, logn, g, c);
+}
+
+// tmp[item] <- sigma_{g_item}(c1 of tab[item].ct): the targets of a key switch with a Galois element per item, for the separate
+// kernels (total = batch k n)
+__global__ void galois_many_kernel(const PrimeDev *primes, int k, const B200GalItem *tab, u64 *tmp, int logn, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long n = 1LL << logn;
+    const long long c = idx & (n - 1);
+    const long long t = idx >> logn;
+    const int r = (int)(t % k);
+    const long long item = t / k;
+    const B200GalItem it = tab[item];
+    galois_coeff(__ldg(&primes[r].p), it.ct + ((long long)k + r) * n, tmp + (item * k + r) * n, logn, it.g, c);
 }
 
 // mode 0: add, 1: sub, 2: negate (b unused)
@@ -803,6 +901,78 @@ __global__ void __launch_bounds__(MAC_NT) plain_mac_kernel(const PrimeDev *prime
 #pragma unroll
         for (int c = 0; c < SZ; c++)
             stg2(out + ((i0 + u) * size + c0 + c) * kn + off, lo[u][c][0], lo[u][c][1]);
+    }
+}
+
+// plain_mac_kernel<2> over several ciphertext vectors with a mask of present terms, for the inner sums of the BSGS linear
+// transform: out[v][i] (at out + v ovs + i ors) = sum_{j < m, present[i][j]} X[v][j] (at X + v xvs + j xjs) * P[i][j].
+// present == nullptr: every term.  An absent term's P and its product are skipped, so its X may be any words.  blockIdx.x runs
+// over (vector, row block), row blocks innermost, so the CTAs of one vector are adjacent and share their X tile.  The
+// arithmetic (lazy 128-bit sums, `lazy` terms between two reductions) is plain_mac_kernel's.
+__global__ void __launch_bounds__(MAC_NT, 2) plain_mac_multi_kernel(const PrimeDev *primes, int k, const u64 *X, long long xjs, long long xvs,
+                                                                 const u64 *P, long long m, long long R, const unsigned char *present,
+                                                                 int lazy, u64 *out, long long ors, long long ovs, int logn)
+{
+    constexpr int SZ = 2;
+    const long long kn = (long long)k << logn;
+    const long long off = ((long long)blockIdx.y * blockDim.x + threadIdx.x) * 2; // r * n + x of the pair
+    if (off >= kn)
+        return;
+    const PrimeDev Q = ld_prime(&primes[(int)(off >> logn)]);
+    const long long rb = (R + MAC_ROWS - 1) / MAC_ROWS, v = (long long)blockIdx.x / rb;
+    const long long i0 = ((long long)blockIdx.x - v * rb) * MAC_ROWS;
+    X += v * xvs;
+    out += v * ovs;
+    u64 lo[MAC_ROWS][SZ][2], hi[MAC_ROWS][SZ][2];
+#pragma unroll
+    for (int u = 0; u < MAC_ROWS; u++)
+#pragma unroll
+        for (int c = 0; c < SZ; c++)
+            lo[u][c][0] = lo[u][c][1] = hi[u][c][0] = hi[u][c][1] = 0;
+    for (long long j0 = 0; j0 < m; j0 += lazy)
+    {
+        const long long j1 = j0 + lazy < m ? j0 + lazy : m;
+        for (long long j = j0; j < j1; j++)
+        {
+            b200_u64x2 x[SZ];
+#pragma unroll
+            for (int c = 0; c < SZ; c++)
+                x[c] = ldg2(X + j * xjs + c * kn + off);
+#pragma unroll
+            for (int u = 0; u < MAC_ROWS; u++)
+            {
+                if (i0 + u >= R)
+                    break;
+                if (present && !present[(i0 + u) * m + j])
+                    continue;
+                const b200_u64x2 p = ldg2(P + ((i0 + u) * m + j) * kn + off);
+#pragma unroll
+                for (int c = 0; c < SZ; c++)
+                {
+                    mac128(x[c].x, p.x, lo[u][c][0], hi[u][c][0]);
+                    mac128(x[c].y, p.y, lo[u][c][1], hi[u][c][1]);
+                }
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < MAC_ROWS; u++)
+#pragma unroll
+            for (int c = 0; c < SZ; c++)
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+                {
+                    lo[u][c][h] = barrett128(lo[u][c][h], hi[u][c][h], Q.p, Q.r0, Q.r1);
+                    hi[u][c][h] = 0;
+                }
+    }
+#pragma unroll
+    for (int u = 0; u < MAC_ROWS; u++)
+    {
+        if (i0 + u >= R)
+            break;
+#pragma unroll
+        for (int c = 0; c < SZ; c++)
+            stg2(out + (i0 + u) * ors + c * kn + off, lo[u][c][0], lo[u][c][1]);
     }
 }
 
@@ -2046,6 +2216,17 @@ struct KsSum
     int m;
 };
 
+// b200_apply_galois_many and the BSGS linear transform through keyswitch_core: item i's target is sigma_{g_i}(c1) of tab[i].ct
+// with key list tab[i].key.  R == 0: each item's result goes to tab[i].dst (ksmoddown_galois_many_kernel); R > 0: the batch is
+// m R items, item j R + r a term of output r, and dst[r] = addend[r] + the sum of its terms (moddown_galois_sum_kernel).
+struct KsMany
+{
+    const B200GalItem *d_tab;           // [batch], device memory
+    const std::vector<B200GalItem> *tab; // the same table on the host: the key groups of the separate kernels' MAC
+    const u64 *addend;                  // R > 0: [R][2][k][n] or nullptr
+    long long R;
+};
+
 // moddown_sum_kernel's term split: R outputs give R n / EB CTAs.  Where those would not fill the GPU (the kernel's resident
 // CTAs per SM times the SM count), the m terms of each output are split into G <= m groups, so that R G n / EB CTAs do; the
 // G partial sums then go through a second launch of the same kernel without a key switch.
@@ -2079,10 +2260,13 @@ static int moddown_sum_groups(b200_ctx *ctx, long long R, int m)
 // the addend (ksmoddown_galois_add_kernel); dst is then [item][2][k][n]
 // sum (base0 / base1 unused): the multiply_relin sums of KsSum (moddown_sum_kernel, with D where given); dst is then
 // [sum->R][2][k][n]
+// many (d, key, base0 / base1 unused): the per-item elements and keys of KsMany.  The cluster kernel reads them from the table
+// (ks_cluster_galois_multi_kernel); otherwise galois_many_kernel writes the targets to scratch, and the MAC runs once per run
+// of consecutive items with one key.  dst is used by the sum mod-down only ([many->R][2][k][n])
 static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_stride, const u64 *key, const u64 *base0,
                           long long base0_stride, const u64 *base1, long long base1_stride, u64 *dst,
                           long long dst_stride, long long batch, cudaStream_t s, const u64 *D = nullptr,
-                          const KsGalois *gal = nullptr, const KsSum *sum = nullptr)
+                          const KsGalois *gal = nullptr, const KsSum *sum = nullptr, const KsMany *many = nullptr)
 {
     if (!ctx->host->using_keyswitching || level < 1)
         return fail(B200_E_LOGIC, "keyswitching is not supported by the context");
@@ -2137,8 +2321,9 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
                 cudaEventCreate(&t1);
                 cudaEventRecord(t0, s);
             }
-            const char *kname = gal ? "ks_cluster_galois_kernel" : "ks_cluster_kernel";
-            const int crc = b200_ks_cluster(ctx->logn, job, d, d_stride, key, Kkey, ks2, k, gal ? gal->ginv : 0u, s);
+            const char *kname = many ? "ks_cluster_galois_multi_kernel" : gal ? "ks_cluster_galois_kernel" : "ks_cluster_kernel";
+            const int crc = many ? b200_ks_cluster_multi(ctx->logn, job, many->d_tab, Kkey, ks2, k, s)
+                                 : b200_ks_cluster(ctx->logn, job, d, d_stride, key, Kkey, ks2, k, gal ? gal->ginv : 0u, s);
             if (crc)
                 return fail(B200_E_CUDA, std::string(kname) + ": " + cudaGetErrorString((cudaError_t)crc));
             if (t0)
@@ -2165,6 +2350,17 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         d = sc1;
         d_stride = (long long)k * n;
     }
+    if (!clustered && many)
+    {
+        u64 *sc1 = nullptr;
+        if ((rc = scr.get((size_t)batch * k * n, &sc1)))
+            return rc;
+        const long long total = batch * k * n;
+        B200_LAUNCH(galois_many_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, many->d_tab, sc1, ctx->logn, total);
+        ctx->launches++;
+        d = sc1;
+        d_stride = (long long)k * n;
+    }
     if (!clustered)
     {
         std::vector<int> prime;
@@ -2182,8 +2378,17 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         if ((rc = launch_ntt<true>(ctx, jd, d, d_stride, ks1, (long long)(k + 1) * k * n, batch, 1, s)))
             return rc;
     }
-    if (!clustered)
+    // the MAC's runs of items with one key: [i0, i0 + cnt) with key `key` (many: the runs of equal tab[i].key)
+    for (long long i0 = 0, cnt = batch; !clustered && i0 < batch; i0 += cnt)
     {
+        if (many)
+        {
+            key = (*many->tab)[i0].key;
+            for (cnt = 1; i0 + cnt < batch && (*many->tab)[i0 + cnt].key == key; cnt++)
+                ;
+        }
+        const u64 *ks1g = ks1 + i0 * (k + 1) * k * n;
+        u64 *ks2g = ks2 + i0 * 2 * (k + 1) * n;
         bool done = false;
 #ifndef B200_EMU_HEADER
         // key tile resident in shared memory (one tiled TMA load per CTA), batch walked inside the CTA: the key is read from
@@ -2200,7 +2405,7 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
                 cudaEventCreate(&t1);
                 cudaEventRecord(t0, s);
             }
-            const int rc2 = b200_ksmac_tma(k, L.fp ? 1 : 0, ctx->d_primes, ctx->d_fp_primes, special, Kkey, ks1, key, ks2, n, batch,
+            const int rc2 = b200_ksmac_tma(k, L.fp ? 1 : 0, ctx->d_primes, ctx->d_fp_primes, special, Kkey, ks1g, key, ks2g, n, cnt,
                                            ctx->sm_count, s);
             if (rc2 > 0)
                 return fail(B200_E_CUDA, std::string("ksmac_tma_kernel: ") + cudaGetErrorString((cudaError_t)rc2));
@@ -2220,15 +2425,15 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
             ;
         else if (L.fp)
         {
-            const long long total = batch * (k + 1) * (n >> 1);
-            DISPATCH_K(k, B200_LAUNCH(ksmac_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_fp_primes, special, Kkey, ks1, key,
-                                      ks2, n, total));
+            const long long total = cnt * (k + 1) * (n >> 1);
+            DISPATCH_K(k, B200_LAUNCH(ksmac_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_fp_primes, special, Kkey, ks1g, key,
+                                      ks2g, n, total));
         }
         else
         {
-            const long long total = batch * (k + 1) * n;
+            const long long total = cnt * (k + 1) * n;
             DISPATCH_K(k, B200_LAUNCH(ksmac_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, ctx->d_fp_primes,
-                                      (int)(L.fp != 0), special, Kkey, ks1, key, ks2, n, total));
+                                      (int)(L.fp != 0), special, Kkey, ks1g, key, ks2g, n, total));
         }
         ctx->launches++;
     }
@@ -2296,7 +2501,18 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
     else
     {
         const long long total = batch * 2 * (n >> 1);
-        if (gal)
+        if (many && many->R > 0)
+        {
+            const long long R = many->R, total2 = R * 2 * (n >> 1);
+            DISPATCH_K(k, B200_LAUNCH(moddown_galois_sum_kernel<KK>, blocks_for(total2, EB), EB, 0, s, ctx->d_primes, special,
+                                      ctx->d_inv_qsp, ks2, many->d_tab, many->addend, dst, (int)(batch / R), R, ctx->logn, total2));
+        }
+        else if (many)
+        {
+            DISPATCH_K(k, B200_LAUNCH(ksmoddown_galois_many_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special,
+                                      ctx->d_inv_qsp, ks2, many->d_tab, ctx->logn, total));
+        }
+        else if (gal)
         {
             DISPATCH_K(k, B200_LAUNCH(ksmoddown_galois_add_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special,
                                       ctx->d_inv_qsp, ks2, gal->in2, gal->addend2, dst, ctx->logn, gal->ginv, total));
@@ -3279,6 +3495,70 @@ int b200_apply_galois_add(b200_ctx *ctx, int level, const uint64_t *in2, uint32_
                           (cudaStream_t)stream, nullptr, &gal);
 }
 
+// g^-1 mod 2n = g^(n-1): the odd residues mod 2n form a group of order n
+static u32 galois_inverse(u64 n, u32 g)
+{
+    const u64 m2 = 2 * n;
+    u64 ginv = 1, base = g;
+    for (u64 e = n - 1; e; e >>= 1, base = base * base % m2)
+        if (e & 1)
+            ginv = ginv * base % m2;
+    return (u32)ginv;
+}
+
+// a host table copied into stream-ordered scratch (the copy from pageable memory is staged before cudaMemcpyAsync returns)
+static int upload_table(Scratch &scr, const void *host, size_t bytes, cudaStream_t s, const void **out)
+{
+    u64 *p = nullptr;
+    int rc;
+    if ((rc = scr.get((bytes + 7) / 8, &p)))
+        return rc;
+    CU_TRY(cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, s));
+    *out = p;
+    return 0;
+}
+
+int b200_apply_galois_many(b200_ctx *ctx, int level, const uint64_t *in2, const uint64_t *src_idx, const uint32_t *elts,
+                           const uint64_t *const *keys, uint64_t *out2, uint64_t batch, void *stream)
+{
+    int rc = check_level(ctx, level);
+    if (rc)
+        return rc;
+    if (!in2 || !elts || !keys || !out2)
+        return fail(B200_E_NULL, "null pointer");
+    if (batch == 0)
+        return 0;
+    const long long n = (long long)ctx->n, w = 2LL * ctx->levels[level].k * n;
+    uint64_t sources = 0;
+    for (uint64_t i = 0; i < batch; i++)
+    {
+        if (!(elts[i] & 1) || elts[i] >= 2 * ctx->n)
+            return fail(B200_E_INVALID, "Galois element is not valid");
+        if (!keys[i])
+            return fail(B200_E_NULL, "null key");
+        sources = std::max(sources, (src_idx ? src_idx[i] : i) + 1);
+    }
+    {
+        const uintptr_t x0 = (uintptr_t)in2, x1 = x0 + (uintptr_t)(sources * w * sizeof(u64));
+        const uintptr_t o0 = (uintptr_t)out2, o1 = o0 + (uintptr_t)(batch * w * sizeof(u64));
+        if (x0 < o1 && o0 < x1)
+            return fail(B200_E_INVALID, "apply_galois_many: out overlaps in");
+    }
+    CU_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    std::vector<B200GalItem> tab(batch);
+    for (uint64_t i = 0; i < batch; i++)
+        tab[i] = B200GalItem{ (const u64 *)in2 + (src_idx ? src_idx[i] : i) * w, (const u64 *)keys[i], (u64 *)out2 + i * w, elts[i],
+                              galois_inverse(ctx->n, elts[i]) };
+    Scratch scr(ctx, s);
+    const B200GalItem *d_tab = nullptr;
+    if ((rc = upload_table(scr, tab.data(), tab.size() * sizeof(B200GalItem), s, (const void **)&d_tab)))
+        return rc;
+    const KsMany many{ d_tab, &tab, nullptr, 0 };
+    return keyswitch_core(ctx, level, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, (long long)batch, s, nullptr, nullptr,
+                          nullptr, &many);
+}
+
 // plain [pb][n] -> out [pb][k][n]: each plaintext lifted to the level's residues and put in NTT form.  monomial != 0 gives
 // the operand multiply_plain_normal multiplies by, with its monomial path (S/evaluator.cpp:1885-1933); monomial == 0 the
 // upper-half lift of transform_to_ntt_inplace(Plaintext &, parms_id) (S/evaluator.cpp:2033-2124).
@@ -3432,6 +3712,161 @@ int b200_multiply_plain_sum(b200_ctx *ctx, int level, const uint64_t *cts, int s
     }
     if ((rc = launch_ntt<false>(ctx, jd, (u64 *)out, kn, (u64 *)out, kn, (long long)R * size, 0, s)))
         return rc;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// Baby-step giant-step slot-wise linear transform of V ciphertexts:
+//     inner_g = sum_{j < b, present[g][j]} multiply_plain(rotate(ct, step j), P[g][j])      (step 0: ct itself)
+//     out     = inner_0 + sum_{g >= 1} rotate(inner_g, giant step g)                          (rows without a present term dropped)
+// per chunk of vectors: the used baby steps as one key switch with a Galois element per item, the forward NTT of the b copies,
+// the masked MAC of all vectors (plain_mac_multi_kernel), the inverse NTT of the G inner sums, and the giant steps as one key
+// switch whose mod-down sums them onto inner_0 (moddown_galois_sum_kernel).  Every hand-off is canonical and sums mod q do not
+// depend on grouping, so the words are those of the rotate / multiply_plain / add chain.  Scratch per chunk is bounded by
+// B200_LINEAR_SCRATCH bytes (default 1 GiB), by chunks of whole vectors.  One vector is never split, so a single vector whose
+// copies, inner sums and key-switch scratch exceed the bound still runs in one chunk (about 10 GB at n = 32768, k = 15,
+// b = G = 64).
+int b200_linear_transform(b200_ctx *ctx, int level, const uint64_t *cts, uint64_t V, int baby, int giant, const uint32_t *elts,
+                          const uint64_t *const *keys, const uint64_t *plain_ntt, const uint8_t *present, uint64_t *out, void *stream)
+{
+    int rc = check_level(ctx, level);
+    if (rc)
+        return rc;
+    if (!cts || !plain_ntt || !out)
+        return fail(B200_E_NULL, "null pointer");
+    if (baby < 1 || giant < 1)
+        return fail(B200_E_INVALID, "baby and giant must be at least 1");
+    const int b = baby, G = giant;
+    std::vector<char> ub(b, 0), ug(G, 0);
+    for (int g = 0; g < G; g++)
+        for (int j = 0; j < b; j++)
+            if (!present || present[(long long)g * b + j])
+                ub[j] = ug[g] = 1;
+    if (std::find(ug.begin(), ug.end(), 1) == ug.end())
+        return fail(B200_E_INVALID, "linear_transform: every term is absent");
+    auto step_ok = [&](int e) -> int {
+        if (!elts || !keys)
+            return fail(B200_E_NULL, "null pointer");
+        if (!(elts[e] & 1) || elts[e] >= 2 * ctx->n)
+            return fail(B200_E_INVALID, "Galois element is not valid");
+        if (!keys[e])
+            return fail(B200_E_NULL, "null key");
+        return 0;
+    };
+    for (int j = 1; j < b; j++)
+        if (ub[j] && (rc = step_ok(j - 1)))
+            return rc;
+    for (int g = 1; g < G; g++)
+        if (ug[g] && (rc = step_ok(b - 1 + g - 1)))
+            return rc;
+    if ((!ctx->host->using_keyswitching || level < 1) &&
+        (std::count(ub.begin() + 1, ub.end(), 1) || std::count(ug.begin() + 1, ug.end(), 1)))
+        return fail(B200_E_LOGIC, "keyswitching is not supported by the context");
+    const long long n = (long long)ctx->n;
+    const LevelHost &Lh = ctx->host->levels[level];
+    const int k = Lh.k;
+    const long long kn = (long long)k * n, w = 2 * kn;
+    {
+        const uintptr_t x0 = (uintptr_t)cts, x1 = x0 + (uintptr_t)(V * w * sizeof(u64));
+        const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (uintptr_t)(V * w * sizeof(u64));
+        if (V && out != cts && x0 < o1 && o0 < x1)
+            return fail(B200_E_INVALID, "out must be cts or not overlap it");
+    }
+    if (V == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int nb = (int)std::count(ub.begin() + 1, ub.end(), 1), ng = (int)std::count(ug.begin() + 1, ug.end(), 1);
+    // scratch words per vector: the b copies, the G inner sums, and the key switches' ks1, ks2 and targets per item
+    const long long per = (long long)(b + G) * w + (long long)(nb + ng) * ((k + 1) * (k + 2) * n + kn);
+    long long budget = 1LL << 30;
+    if (const char *e = std::getenv("B200_LINEAR_SCRATCH"))
+        budget = std::max(1LL, atoll(e));
+    const long long chunk = std::max(1LL, budget / (per * (long long)sizeof(u64)));
+    JobDesc jd;
+    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+        return rc;
+    int bits = 0; // terms between two reductions of the MAC, as in b200_multiply_plain_sum
+    for (int r = 0; r < k; r++)
+        bits = std::max(bits, 64 - __builtin_clzll(ctx->host->primes[Lh.q_idx[r]].mod.p));
+    const int lazy = bits <= 60 ? 256 : 1 << (128 - 2 * bits);
+    std::vector<unsigned char> mask;
+    if (present)
+        mask.assign(present, present + (long long)G * b);
+    for (uint64_t v0 = 0; v0 < V; v0 += chunk)
+    {
+        const long long Vc = (long long)std::min<uint64_t>(chunk, V - v0);
+        const u64 *ct = (const u64 *)cts + v0 * w;
+        u64 *o = (u64 *)out + v0 * w;
+        Scratch scr(ctx, s);
+        u64 *X = nullptr, *inner = nullptr; // [b][Vc][2][k][n], [G][Vc][2][k][n]
+        if ((rc = scr.get((size_t)b * Vc * w, &X)) || (rc = scr.get((size_t)G * Vc * w, &inner)))
+            return rc;
+        // baby steps: X[j] = rotate(ct, step j) for the used steps, one key switch; X[0] = NTT(ct).  The copies of unused steps
+        // are neither written nor read (the MAC skips absent terms' products)
+        if (ub[0])
+        {
+            if ((rc = launch_ntt<true>(ctx, jd, ct, kn, X, kn, 2 * Vc, 0, s)))
+                return rc;
+        }
+        if (nb)
+        {
+            std::vector<B200GalItem> tab;
+            for (int j = 1; j < b; j++)
+                if (ub[j])
+                    for (long long v = 0; v < Vc; v++)
+                        tab.push_back(B200GalItem{ ct + v * w, (const u64 *)keys[j - 1], X + (j * Vc + v) * w, elts[j - 1],
+                                                   galois_inverse(ctx->n, elts[j - 1]) });
+            const B200GalItem *d_tab = nullptr;
+            if ((rc = upload_table(scr, tab.data(), tab.size() * sizeof(B200GalItem), s, (const void **)&d_tab)))
+                return rc;
+            const KsMany many{ d_tab, &tab, nullptr, 0 };
+            if ((rc = keyswitch_core(ctx, level, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, (long long)tab.size(), s, nullptr,
+                                     nullptr, nullptr, &many)))
+                return rc;
+        }
+        // forward NTT of the rotated copies: one launch per run of consecutive used steps (one run when every step is used)
+        for (int j0 = 1, j1; j0 < b; j0 = j1)
+        {
+            for (j1 = j0 + 1; j1 < b && ub[j1] == ub[j0]; j1++)
+                ;
+            if (ub[j0] && (rc = launch_ntt<true>(ctx, jd, X + j0 * Vc * w, kn, X + j0 * Vc * w, kn, 2 * Vc * (j1 - j0), 0, s)))
+                return rc;
+        }
+        // inner[g][v] = sum_j X[j][v] P[g][j] in the NTT domain, all vectors in one launch, then back to coefficient form
+        {
+            const unsigned char *d_mask = nullptr;
+            if (present && (rc = upload_table(scr, mask.data(), mask.size(), s, (const void **)&d_mask)))
+                return rc;
+            const dim3 grid((unsigned)(Vc * ((G + MAC_ROWS - 1) / MAC_ROWS)), blocks_for(kn / 2, MAC_NT));
+            B200_LAUNCH(plain_mac_multi_kernel, grid, MAC_NT, 0, s, ctx->d_primes, k, (const u64 *)X, Vc * w, w, (const u64 *)plain_ntt,
+                        (long long)b, (long long)G, d_mask, lazy, inner, Vc * w, w, ctx->logn);
+            ctx->launches++;
+        }
+        if ((rc = launch_ntt<false>(ctx, jd, inner, kn, inner, kn, 2 * Vc * G, 0, s)))
+            return rc;
+        // giant steps: out = inner_0 + sum_g rotate(inner_g), one key switch whose mod-down sums the terms
+        if (ng == 0)
+        {
+            CU_TRY(cudaMemcpyAsync(o, inner, (size_t)Vc * w * sizeof(u64), cudaMemcpyDeviceToDevice, s));
+            continue;
+        }
+        std::vector<B200GalItem> tab;
+        for (int g = 1; g < G; g++)
+            if (ug[g])
+            {
+                const int e = b - 1 + g - 1;
+                for (long long v = 0; v < Vc; v++)
+                    tab.push_back(B200GalItem{ inner + (g * Vc + v) * w, (const u64 *)keys[e], nullptr, elts[e], galois_inverse(ctx->n, elts[e]) });
+            }
+        const B200GalItem *d_tab = nullptr;
+        if ((rc = upload_table(scr, tab.data(), tab.size() * sizeof(B200GalItem), s, (const void **)&d_tab)))
+            return rc;
+        const KsMany many{ d_tab, &tab, ug[0] ? inner : nullptr, Vc };
+        if ((rc = keyswitch_core(ctx, level, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, o, 0, (long long)tab.size(), s, nullptr, nullptr,
+                                 nullptr, &many)))
+            return rc;
+    }
     CU_TRY(cudaGetLastError());
     return 0;
 }

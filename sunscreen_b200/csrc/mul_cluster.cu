@@ -151,9 +151,10 @@ __device__ __forceinline__ KsPlace ks_place(int k)
 // GAL: the target is sigma_g(d) for the Galois element g with g^-1 mod 2n = ginv.  Digit J is gathered from d by the first
 // forward pass and negated mod q_J where the automorphism flips the sign, before its reduction mod p_I: the digits are the
 // integers the separate galois_kernel would have written, so every later word is unchanged.
-template <int LOGN, bool GAL>
+// MULTI (with GAL): item i's target is sigma_{g_i}(c1) of tab[i].ct with tab[i]'s key; d, d_stride, key and ginv are unused.
+template <int LOGN, bool GAL, bool MULTI = false>
 __device__ __forceinline__ void ks_cluster_body(const NttJob &job, const u64 *d, long long d_stride, const u64 *key, int key_rows,
-                                                u64 *ks2, int k, unsigned ginv)
+                                                u64 *ks2, int k, unsigned ginv, const B200GalItem *tab = nullptr)
 {
     extern __shared__ u64 mc_sm[];
     constexpr int N = 1 << LOGN;
@@ -164,8 +165,12 @@ __device__ __forceinline__ void ks_cluster_body(const NttJob &job, const u64 *d,
         const NttPrimeFp PF = job.fprimes[job.slot_prime[w.I]];
         const NttPrime PI_ = job.primes[job.slot_prime[w.I]];
         // digit J of the target, reduced mod p_I by the first pass (job.reduce_input)
-        const u64 *dj = d + w.item * d_stride + (long long)w.J * N;
-        if constexpr (GAL)
+        const u64 *dj = MULTI ? nullptr : d + w.item * d_stride + (long long)w.J * N;
+        if constexpr (MULTI)
+            NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR | 8192>::run(job, PF, PI_, tab[w.item].ct + (long long)(k + w.J) * N, nullptr, smd,
+                                                                    tid, w.item, w.I, nullptr, tab[w.item].ginv,
+                                                                    job.primes[job.slot_prime[w.J]].p);
+        else if constexpr (GAL)
             NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR | 8192>::run(job, PF, PI_, dj, nullptr, smd, tid, w.item, w.I, nullptr, ginv,
                                                                     job.primes[job.slot_prime[w.J]].p);
         else
@@ -185,7 +190,7 @@ __device__ __forceinline__ void ks_cluster_body(const NttJob &job, const u64 *d,
         asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r1) : "r"(base), "r"(1));
         // key[J][c][residue][coeff]: the special prime's row is the last key residue
         const long long kstride = (long long)key_rows * N;
-        const u64 *kr = key + (long long)(w.I < k ? w.I : key_rows - 1) * N + tid;
+        const u64 *kr = (MULTI ? tab[w.item].key : key) + (long long)(w.I < k ? w.I : key_rows - 1) * N + tid;
         // U chunks per round: their k remote loads and 2k key loads are issued per digit together (n = 4096: two, as in
         // mul_cluster_kernel a wider round makes ptxas spill)
         constexpr int CH = N / NT, U = LOGN >= 13 ? 4 : 2;
@@ -262,6 +267,13 @@ __global__ void __launch_bounds__(NT, 3) ks_cluster_galois_kernel(const NttJob j
 }
 
 template <int LOGN>
+__global__ void __launch_bounds__(NT, 3) ks_cluster_galois_multi_kernel(const NttJob job, const B200GalItem *tab, int key_rows, u64 *ks2,
+                                                                        int k)
+{
+    ks_cluster_body<LOGN, true, true>(job, nullptr, 0, nullptr, key_rows, ks2, k, 0, tab);
+}
+
+template <int LOGN>
 cudaLaunchConfig_t config(long long clusters, cudaLaunchAttribute *at, cudaStream_t s, int csize = CLUSTER)
 {
     at[0].id = cudaLaunchAttributeClusterDimension;
@@ -325,14 +337,33 @@ int b200_ks_cluster_setup(int logn, int k, int *active)
     *active = 0;
     if (k < 2 || k > 8)
         return 0;
-    // both variants: the same shared memory, and the register bound of __launch_bounds__; the smaller count of the two
-    int plain = 0, gal = 0, rc = 0;
-    if (logn == 12 && !(rc = setup<12>(ks_cluster_kernel<12>, k, &plain)))
-        rc = setup<12>(ks_cluster_galois_kernel<12>, k, &gal);
-    if (logn == 13 && !(rc = setup<13>(ks_cluster_kernel<13>, k, &plain)))
-        rc = setup<13>(ks_cluster_galois_kernel<13>, k, &gal);
-    *active = rc ? 0 : std::min(plain, gal);
+    // all three variants: the same shared memory, and the register bound of __launch_bounds__; the smallest count of them
+    int plain = 0, gal = 0, multi = 0, rc = 0;
+    if (logn == 12 && !(rc = setup<12>(ks_cluster_kernel<12>, k, &plain)) && !(rc = setup<12>(ks_cluster_galois_kernel<12>, k, &gal)))
+        rc = setup<12>(ks_cluster_galois_multi_kernel<12>, k, &multi);
+    if (logn == 13 && !(rc = setup<13>(ks_cluster_kernel<13>, k, &plain)) && !(rc = setup<13>(ks_cluster_galois_kernel<13>, k, &gal)))
+        rc = setup<13>(ks_cluster_galois_multi_kernel<13>, k, &multi);
+    *active = rc ? 0 : std::min(plain, std::min(gal, multi));
     return rc;
+}
+
+int b200_ks_cluster_multi(int logn, const NttJob &job, const B200GalItem *tab, int key_rows, u64 *ks2, int k, void *stream)
+{
+    cudaLaunchAttribute at[1];
+    const long long clusters = job.items * (k + 1);
+    if (k < 2 || k > 8)
+        return (int)cudaErrorInvalidValue;
+    if (logn == 12)
+    {
+        const cudaLaunchConfig_t cfg = config<12>(clusters, at, (cudaStream_t)stream, k);
+        return (int)cudaLaunchKernelEx(&cfg, ks_cluster_galois_multi_kernel<12>, job, tab, key_rows, ks2, k);
+    }
+    if (logn == 13)
+    {
+        const cudaLaunchConfig_t cfg = config<13>(clusters, at, (cudaStream_t)stream, k);
+        return (int)cudaLaunchKernelEx(&cfg, ks_cluster_galois_multi_kernel<13>, job, tab, key_rows, ks2, k);
+    }
+    return (int)cudaErrorInvalidValue;
 }
 
 int b200_ks_cluster(int logn, const NttJob &job, const u64 *d, long long d_stride, const u64 *key, int key_rows, u64 *ks2, int k,

@@ -21,3 +21,6 @@ int b200_ks_cluster_setup(int logn, int k, int *active);
 // digit gathered from d and negated mod q_J as galois_kernel does (ks_cluster_galois_kernel).  Returns a cudaError_t.
 int b200_ks_cluster(int logn, const NttJob &job, const u64 *d, long long d_stride, const u64 *key, int key_rows, u64 *ks2, int k,
                     unsigned galois_inv, void *stream);
+// The same with a Galois element and a key per item (ks_cluster_galois_multi_kernel): item i's target is sigma_{g_i}(c1) of
+// tab[i].ct ([2][k][n]), its key list tab[i].key; tab [job.items] is in device memory.  Returns a cudaError_t.
+int b200_ks_cluster_multi(int logn, const NttJob &job, const B200GalItem *tab, int key_rows, u64 *ks2, int k, void *stream);

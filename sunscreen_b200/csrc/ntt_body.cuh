@@ -35,6 +35,17 @@ struct NttPrime
 
 struct NttPrimeFp; // ntt_fp_body.cuh
 
+// One item of a key switch whose items carry their own Galois element and key (b200_apply_galois_many, the BSGS linear
+// transform): the source ciphertext [2][k][n], the key list [J][2][key_rows][n], where the per-item mod-down writes the
+// result ([2][k][n]; unused by the summing mod-down), the element g and g^-1 mod 2n.
+struct B200GalItem
+{
+    const u64 *ct;
+    const u64 *key;
+    u64 *dst;
+    unsigned g, ginv;
+};
+
 // One launch = `items` x `slots` residue polynomials.
 struct NttJob
 {

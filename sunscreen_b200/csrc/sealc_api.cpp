@@ -2542,6 +2542,187 @@ long B200_Evaluator_RotateSumBatch(void *p, uint64_t count, void **encs, int nst
     });
 }
 
+namespace
+{
+// the Galois element of RotateRows(step) and its key list's index; a step without its own key is refused (no NAF parts)
+size_t row_step_key(Context_ *c, KSwitchKeys_ &keys, int step, uint32_t *elt)
+{
+    if (b200_galois_elt_from_step(c->dev, step, elt))
+        throw InvalidArg("step count too large");
+    const size_t idx = (*elt - 1) >> 1;
+    if (idx >= keys.keys.size() || keys.keys[idx].empty())
+        throw InvalidArg("Galois key not present");
+    check_keys(c, keys, idx);
+    return idx;
+}
+} // namespace
+
+// Row rotations by a step per item.  The items are gathered in the order of their Galois elements (step 0 last, a copy), so
+// each element's items are one run of one key, and rotated by one b200_apply_galois_many; the results are scattered back to
+// their destinations.  Every operand is gathered before the scatter, so destinations may alias encrypteds.
+long B200_Evaluator_RotateRowsStepsBatch(void *p, uint64_t count, void **encs, const int *steps, void *galois_keys, void **dsts)
+{
+    NULLRET(p);
+    NULLRET(encs);
+    NULLRET(steps);
+    NULLRET(galois_keys);
+    NULLRET(dsts);
+    auto *c = ((Evaluator_ *)p)->ctx;
+    auto &keys = *(KSwitchKeys_ *)galois_keys;
+    return guard([&] {
+        if (count == 0)
+            return;
+        if (!c->using_batching)
+            throw LogicErr("encryption parameters do not support batching");
+        batch_handles(count, { encs, dsts });
+        batch_item_words(c, encs);
+        for (uint64_t i = 0; i < count; i++)
+        {
+            auto &a = *(Ciphertext_ *)encs[i];
+            data_level(c, a, "encrypted is not valid for encryption parameters");
+            if (a.is_ntt_form || a.size != 2)
+                throw InvalidArg("batch items must be size-2 ciphertexts at the same level");
+        }
+        if (!c->using_keyswitching)
+            throw LogicErr("keyswitching is not supported by the context");
+        if (keys.parms_id != c->ids[0])
+            throw InvalidArg("galois_keys is not valid for encryption parameters");
+        std::vector<uint32_t> elt(count, 0);
+        std::vector<size_t> idx(count, 0);
+        for (uint64_t i = 0; i < count; i++)
+            if (steps[i] != 0)
+                idx[i] = row_step_key(c, keys, steps[i], &elt[i]);
+        std::vector<uint64_t> order(count);
+        for (uint64_t i = 0; i < count; i++)
+            order[i] = i;
+        std::stable_sort(order.begin(), order.end(), [&](uint64_t x, uint64_t y) {
+            return (elt[x] ? elt[x] : UINT32_MAX) < (elt[y] ? elt[y] : UINT32_MAX);
+        });
+        std::vector<void *> src(count), dst(count);
+        for (uint64_t i = 0; i < count; i++)
+        {
+            src[i] = encs[order[i]];
+            dst[i] = dsts[order[i]];
+        }
+        uint64_t m = 0; // items with a rotation
+        while (m < count && elt[order[m]])
+            m++;
+        OpScope scope(c);
+        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        const u64 w = batch_item_words(c, encs);
+        BatchSlab A(c, count * w), O(c, count * w);
+        u64 k = 0;
+        const int lv = batch_gather(c, count, src.data(), A, k);
+        if (m)
+        {
+            std::vector<uint32_t> el(m);
+            std::vector<const uint64_t *> kp(m);
+            for (uint64_t i = 0; i < m; i++)
+            {
+                el[i] = elt[order[i]];
+                kp[i] = keys.flat_dev(c, idx[order[i]], (int)k);
+            }
+            dev_check(b200_apply_galois_many(c->dev, lv, A.w(), nullptr, el.data(), kp.data(), O.w(), m, cur_stream()));
+        }
+        if (m < count)
+            dev_check(b200_memcpy_d2d(c->dev, O.w() + m * w, A.w() + m * w, (count - m) * w * sizeof(u64), cur_stream()));
+        batch_scatter(c, count, dst.data(), O, ((Ciphertext_ *)encs[0])->parms_id, k, lv);
+    });
+}
+
+// Baby-step giant-step linear transform: the chain of B200_Evaluator_LinearTransform (b200_sealc.h) as one
+// b200_linear_transform over the gathered ciphertexts, with the present plaintexts lifted to NTT form once per call.  Every
+// plaintext, step and key is checked before any work; operands are gathered before the scatter, so destinations may alias
+// encrypteds.
+long B200_Evaluator_LinearTransform(void *p, uint64_t count, void **encs, uint64_t baby, uint64_t giant, void **plains,
+                                    void *galois_keys, void **dsts)
+{
+    NULLRET(p);
+    NULLRET(encs);
+    NULLRET(plains);
+    NULLRET(galois_keys);
+    NULLRET(dsts);
+    auto *c = ((Evaluator_ *)p)->ctx;
+    auto &keys = *(KSwitchKeys_ *)galois_keys;
+    return guard([&] {
+        if (count == 0)
+            return;
+        if (baby == 0 || giant == 0 || baby > (1u << 20) || giant > (1u << 20))
+            throw InvalidArg("baby and giant must be at least 1");
+        if (!c->using_batching)
+            throw LogicErr("encryption parameters do not support batching");
+        batch_handles(count, { encs, dsts });
+        batch_item_words(c, encs);
+        for (uint64_t i = 0; i < count; i++)
+        {
+            auto &a = *(Ciphertext_ *)encs[i];
+            data_level(c, a, "encrypted is not valid for encryption parameters");
+            if (a.is_ntt_form || a.size != 2)
+                throw InvalidArg("batch items must be size-2 ciphertexts at the same level");
+        }
+        const size_t n = c->parms.n;
+        const uint64_t terms = baby * giant;
+        std::vector<uint8_t> present(terms, 0);
+        std::vector<char> ub(baby, 0), ug(giant, 0);
+        std::vector<u64> host(terms * n, 0);
+        for (uint64_t t = 0; t < terms; t++)
+        {
+            if (!plains[t])
+                continue;
+            std::vector<u64> pv = padded_plain(c, *(Plaintext_ *)plains[t], false);
+            if (c->check_transparent && std::all_of(pv.begin(), pv.end(), [](u64 x) { return x == 0; }))
+                throw LogicErr("result ciphertext is transparent");
+            std::copy(pv.begin(), pv.end(), host.begin() + t * n);
+            present[t] = 1;
+            ub[t % baby] = ug[t / baby] = 1;
+        }
+        if (std::find(present.begin(), present.end(), 1) == present.end())
+            throw InvalidArg("every term is absent");
+        const uint64_t ns = baby - 1 + giant - 1;
+        std::vector<uint32_t> elts(std::max<uint64_t>(ns, 1), 0);
+        std::vector<size_t> idx(std::max<uint64_t>(ns, 1), 0);
+        bool rotates = false;
+        for (uint64_t j = 1; j < baby; j++)
+            rotates = rotates || ub[j];
+        for (uint64_t g = 1; g < giant; g++)
+            rotates = rotates || ug[g];
+        if (rotates)
+        {
+            if (!c->using_keyswitching)
+                throw LogicErr("keyswitching is not supported by the context");
+            if (keys.parms_id != c->ids[0])
+                throw InvalidArg("galois_keys is not valid for encryption parameters");
+        }
+        for (uint64_t j = 1; j < baby; j++)
+            if (ub[j])
+                idx[j - 1] = row_step_key(c, keys, (int)j, &elts[j - 1]);
+        for (uint64_t g = 1; g < giant; g++)
+            if (ug[g])
+            {
+                if (g * baby >= n / 2)
+                    throw InvalidArg("step count too large");
+                idx[baby - 1 + g - 1] = row_step_key(c, keys, (int)(g * baby), &elts[baby - 1 + g - 1]);
+            }
+        OpScope scope(c);
+        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        const u64 w = batch_item_words(c, encs);
+        BatchSlab A(c, count * w), O(c, count * w);
+        u64 k = 0;
+        const int lv = batch_gather(c, count, encs, A, k);
+        std::vector<const uint64_t *> kp(std::max<uint64_t>(ns, 1), nullptr);
+        for (uint64_t e = 0; e < ns; e++)
+            if (elts[e])
+                kp[e] = keys.flat_dev(c, idx[e], (int)k);
+        BatchSlab Pc(c, terms * n), Pn(c, terms * k * n);
+        dev_check(b200_memcpy_h2d(c->dev, Pc.p, host.data(), host.size() * sizeof(u64), cur_stream()));
+        dev_check(b200_plain_to_ntt(c->dev, lv, Pc.w(), terms, Pn.w(), B200_PLAIN_NTT_MULTIPLY, cur_stream()));
+        dev_check(b200_linear_transform(c->dev, lv, A.w(), count, (int)baby, (int)giant, elts.data(), kp.data(), Pn.w(),
+                                        present.data(), O.w(), cur_stream()));
+        scope.wait(); // `host` is read by the copy above
+        batch_scatter(c, count, dsts, O, ((Ciphertext_ *)encs[0])->parms_id, k, lv);
+    });
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Decryptor
 // ---------------------------------------------------------------------------------------------------------

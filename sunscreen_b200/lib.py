@@ -79,6 +79,8 @@ _SIGS = {
     "b200_multiply_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
     "b200_plain_to_ntt": [vp, C.c_int, vp, u64, vp, C.c_int, vp],
     "b200_multiply_plain_sum": [vp, C.c_int, vp, C.c_int, u64, vp, u64, vp, vp],
+    "b200_apply_galois_many": [vp, C.c_int, vp, vp, vp, vp, vp, u64, vp],
+    "b200_linear_transform": [vp, C.c_int, vp, u64, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp],
     "b200_add_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
     "b200_sub_plain": [vp, C.c_int, vp, C.c_int, vp, u64, vp, u64, vp],
     "b200_mod_switch_to_next": [vp, C.c_int, vp, C.c_int, vp, u64, vp],
@@ -271,6 +273,30 @@ class B200Context:
         """out2 = addend2 + apply_galois(in2, elt) (addend2 None: no addend); addend2 may be in2 or out2, out2 must not overlap in2."""
         self.L.call("b200_apply_galois_add", self.h, self._lv(level), vp(ptr(in2)), C.c_uint32(elt), vp(ptr(key)),
                     vp(ptr(addend2)), vp(ptr(out2)), u64(batch), vp(stream))
+
+    def apply_galois_many(self, in2, src_idx, elts, keys, out2, level=None, stream=None):
+        """out2[i] = apply_galois(in2[src_idx[i]], elts[i]) with key list keys[i] (src_idx None: item i), one key switch for
+        all items; out2 must not overlap the sources."""
+        batch = len(elts)
+        src = (u64 * max(batch, 1))(*([int(x) for x in src_idx] if src_idx is not None else []))
+        el = (C.c_uint32 * max(batch, 1))(*[int(e) for e in elts])
+        ks = (vp * max(batch, 1))(*[ptr(key) for key in keys])
+        self.L.call("b200_apply_galois_many", self.h, self._lv(level), vp(ptr(in2)), src if src_idx is not None else None, el, ks,
+                    vp(ptr(out2)), u64(batch), vp(stream))
+
+    def linear_transform(self, cts, V, baby, giant, elts, keys, plain_ntt, out, present=None, level=None, stream=None):
+        """Baby-step giant-step slot-wise linear transform (see bsgs_plain_vectors): cts, out [V][2][k][n]; elts, keys the
+        baby - 1 baby-step then giant - 1 giant-step elements and device key lists (None where no present term uses the step);
+        plain_ntt [giant][baby][k][n] from plain_to_ntt(rule=PLAIN_NTT_MULTIPLY); present [giant][baby] booleans or None."""
+        ns = baby - 1 + giant - 1
+        el = (C.c_uint32 * max(ns, 1))(*[int(e or 0) for e in elts])
+        ks = (vp * max(ns, 1))(*[ptr(key) for key in keys])
+        pr = None
+        if present is not None:
+            flat = [1 if x else 0 for row in present for x in row]
+            pr = (C.c_uint8 * len(flat))(*flat)
+        self.L.call("b200_linear_transform", self.h, self._lv(level), vp(ptr(cts)), u64(V), C.c_int(baby), C.c_int(giant), el, ks,
+                    vp(ptr(plain_ntt)), pr, vp(ptr(out)), vp(stream))
 
     def multiply_plain(self, a, size, plain, plain_batch, out, batch, level=None, stream=None):
         self.L.call("b200_multiply_plain", self.h, self._lv(level), vp(ptr(a)), C.c_int(size), vp(ptr(plain)),
