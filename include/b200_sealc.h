@@ -325,6 +325,21 @@ SEAL_C_FUNC B200_Evaluator_RotateRowsStepsBatch(void *thisptr, uint64_t count, v
 SEAL_C_FUNC B200_Evaluator_LinearTransform(void *thisptr, uint64_t count, void **encrypteds, uint64_t baby, uint64_t giant, void **plains,
                                            void *galois_keys, void **destinations);
 
+/* ---- debug aids (tests only; not part of the seal_fhe surface) ---- */
+/* `count` (1 ... 64) per-handle calls of one kind run as if they had arrived together at the combiner: kind 0
+   Evaluator_Multiply(a[i], b[i]), 1 Evaluator_Relinearize(a[i], keys), 2 Evaluator_ApplyGalois(a[i], galois_elt, keys) as
+   Evaluator_RotateRows / RotateColumns combine it; results go to destinations[i], HRESULTs to hresults[i].  Every item is
+   validated as its call validates it, then the combinable ones run as one leader's batch (compatible items together) on
+   the calling thread, so the batch size and the graph state it meets are known.  COR_E_INVALIDOPERATION when combining is
+   off (B200_NO_COMBINE). */
+SEAL_C_FUNC B200_Evaluator_CombinedBatchDebug(void *thisptr, int kind, uint64_t count, void **encrypteds1, void **encrypteds2,
+                                              void *keys, uint32_t galois_elt, void **destinations, long *hresults);
+/* counts of what the combiner did with its batches, summed over the context's lanes: out[0] first sights of a graph shape
+   (run kernel by kernel), [1] captures, [2] refused captures, [3] graph replays, [4] LRU evictions of a lane's graph,
+   [5] batches run without a graph (graphs off, an operand that is also a destination of another shape, or a shape whose
+   capture was refused) */
+SEAL_C_FUNC B200_Context_GraphStatsDebug(void *context, uint64_t *out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -164,7 +164,10 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
 {
     const size_t N = batch.size();
     if (N == 1 && !c->use_graphs)
+    {
+        c->graph_stats[Context_::GS_NO_GRAPH]++;
         return combine_run_one(c, *batch[0]);
+    }
     CombineReq &r0 = *batch[0];
     try
     {
@@ -239,6 +242,7 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
                 ((volatile uint32_t *)flags)[i] = 0;
         if (reshaped_alias || !c->use_graphs)
         {
+            c->graph_stats[Context_::GS_NO_GRAPH]++;
             if (NP != N) // (this branch runs unpadded: second operands sit right behind the first N)
                 for (size_t i = 0; i < N && operands == 2; i++)
                     tab[N + i] = const_cast<u64 *>(batch[i]->b->dev_ptr(c));
@@ -271,8 +275,10 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
                     g = &e;
             if (!g)
             { // first sight of this shape on this lane: run it kernel by kernel (this also warms every cache the sequence touches)
+                c->graph_stats[Context_::GS_FIRST]++;
                 if ((int)lane.graphs.size() >= Context_::GRAPHS_PER_LANE)
                 {
+                    c->graph_stats[Context_::GS_EVICT]++;
                     size_t old = 0;
                     for (size_t i = 1; i < lane.graphs.size(); i++)
                         if (lane.graphs[i].stamp < lane.graphs[old].stamp)
@@ -287,9 +293,13 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
             else
             {
                 g->stamp = ++lane.clock;
-                if (!g->exec)
+                if (g->exec)
+                    c->graph_stats[Context_::GS_REPLAY]++;
+                else if (g->kind < 0)
+                    c->graph_stats[Context_::GS_NO_GRAPH]++;
+                else
                 { // second use: capture the sequence; from now on one graph launch replaces its ~10 kernel launches
-                    if (g->kind >= 0 && b200_capture_begin(c->dev, cur_stream()) == 0)
+                    if (b200_capture_begin(c->dev, cur_stream()) == 0)
                     {
                         const int rc = enqueue();
                         void *exec = nullptr;
@@ -303,6 +313,7 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
                         }
                         g->exec = exec;
                     }
+                    c->graph_stats[g->exec ? Context_::GS_CAPTURE : Context_::GS_REFUSED]++;
                 }
                 if (g->exec)
                     dev_check(b200_graph_launch(c->dev, g->exec, cur_stream()));
@@ -324,8 +335,13 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
     }
 }
 
+// B200_Evaluator_CombinedBatchDebug: the requests its items' validation would submit are collected here instead
+static thread_local std::vector<CombineReq> *tl_collect = nullptr;
+
 static void combine_submit(Context_ *c, CombineReq &req)
 {
+    if (tl_collect)
+        return tl_collect->push_back(req);
     Context_::Combiner &cb = c->comb[req.kind];
     std::unique_lock<std::mutex> lk(cb.m);
     cb.pending.push_back(&req);
@@ -2141,6 +2157,78 @@ long B200_Ciphertext_GetWordsBatch(void *context, uint64_t count, void **cts, ui
         dev_check(b200_memcpy_d2h(c->dev, words, S.p, count * w * sizeof(u64), cur_stream()));
         scope.wait(); // context mutex released while the copy runs
     });
+}
+
+// Test aid: what a combiner leader runs for `count` per-handle calls that arrived together, on the calling thread and
+// without thread timing.  Each item goes through its per-handle call's validation; the validated requests run as the
+// leader would take them (compatible ones as one batch, in item order) and each item gets its own HRESULT.
+long B200_Evaluator_CombinedBatchDebug(void *p, int kind, uint64_t count, void **a, void **b, void *keys, uint32_t galois_elt,
+                                       void **dsts, long *hresults)
+{
+    NULLRET(p);
+    NULLRET(a);
+    NULLRET(dsts);
+    NULLRET(hresults);
+    auto *c = ((Evaluator_ *)p)->ctx;
+    if (kind < 0 || kind >= Context_::NCOMB || count == 0 || count > (uint64_t)Context_::COMBINE_MAX || (kind == 0 && !b) ||
+        (kind != 0 && !keys))
+        return E_INVALIDARG_;
+    if (!c->combine || tl_scope)
+        return COR_E_INVALIDOPERATION_; // no combiner to drive
+    std::vector<CombineReq> reqs;
+    std::vector<uint64_t> owner; // item of each collected request
+    reqs.reserve(count);
+    for (uint64_t i = 0; i < count; i++)
+    {
+        if (!a[i] || !dsts[i] || (kind == 0 && !b[i]))
+        {
+            hresults[i] = E_POINTER_;
+            continue;
+        }
+        auto &A = *(Ciphertext_ *)a[i], &D = *(Ciphertext_ *)dsts[i];
+        const size_t before = reqs.size();
+        tl_collect = &reqs;
+        hresults[i] = guard([&] { // an item its per-handle call would not combine runs here, as that call does
+            if (kind == 0)
+                op_multiply(c, A, *(Ciphertext_ *)b[i], D, false);
+            else if (kind == 1)
+                op_relinearize(c, A, *(KSwitchKeys_ *)keys, D);
+            else if (!galois_combined(c, A, galois_elt, *(KSwitchKeys_ *)keys, D))
+            {
+                OpScope scope(c);
+                op_galois(c, A, galois_elt, *(KSwitchKeys_ *)keys, D);
+            }
+        });
+        tl_collect = nullptr;
+        if (reqs.size() > before)
+            owner.push_back(i);
+    }
+    std::vector<CombineReq *> pending;
+    for (auto &r : reqs)
+        pending.push_back(&r);
+    while (!pending.empty())
+    {
+        std::vector<CombineReq *> batch{ pending[0] }, rest;
+        for (size_t j = 1; j < pending.size(); j++)
+            (pending[j]->compatible(*pending[0]) ? batch : rest).push_back(pending[j]);
+        combine_run_batch(c, batch);
+        pending.swap(rest);
+    }
+    for (size_t j = 0; j < reqs.size(); j++)
+        hresults[owner[j]] = guard([&] {
+            if (reqs[j].err)
+                std::rethrow_exception(reqs[j].err);
+        });
+    return S_OK_;
+}
+long B200_Context_GraphStatsDebug(void *context, uint64_t *out)
+{
+    NULLRET(context);
+    NULLRET(out);
+    auto *c = (Context_ *)context;
+    for (int i = 0; i < Context_::GS_COUNT; i++)
+        out[i] = c->graph_stats[i].load();
+    return S_OK_;
 }
 
 long B200_Evaluator_MultiplyRelinBatch(void *p, uint64_t count, void **e1, void **e2, void *relin_keys, void **dsts)

@@ -145,6 +145,11 @@ struct Context_
     };
     static const int GRAPHS_PER_LANE = 48;
     bool use_graphs = true; // B200_NO_GRAPHS=1: enqueue the kernels one by one
+    // what the combining layer did with each batch, summed over the lanes (B200_Context_GraphStatsDebug): a shape's first
+    // sight (kernel by kernel), its capture, a capture that was refused, a replay, an LRU eviction, and a batch that ran
+    // without a graph (graphs off, a reshaped alias, or a shape whose capture was refused before)
+    enum { GS_FIRST, GS_CAPTURE, GS_REFUSED, GS_REPLAY, GS_EVICT, GS_NO_GRAPH, GS_COUNT };
+    std::atomic<uint64_t> graph_stats[GS_COUNT] = {};
     // B200_BLOCKING_WAITS=1: the batch seams sleep on a blocking-sync event instead of spinning in cudaStreamSynchronize.  Off by
     // default: the sleeping wait was measured to halve the throughput of the chunked host-buffer pipeline (wake-up latency
     // of the order of a chunk's run time); it exists for hosts where caller threads outnumber the cores the process is granted.

@@ -171,6 +171,23 @@ class SealcContext:
         self.S.call("Evaluator_AddMany", self.ev, u64(len(cts)), arr, d)
         return d
 
+    # debug aids of include/b200_sealc.h
+    def combined_batch(self, kind, a, b=None, keys=None, galois_elt=0, dsts=None):
+        """B200_Evaluator_CombinedBatchDebug -> (destinations, per-item HRESULTs); the call's own HRESULT must be S_OK"""
+        N = len(a)
+        dsts = dsts or [self._dst() for _ in range(N)]
+        hr = (C.c_long * N)()
+        arr = lambda hs: (vp * N)(*hs)
+        self.S.call("B200_Evaluator_CombinedBatchDebug", self.ev, C.c_int(kind), u64(N), arr(a), arr(b) if b else None, keys,
+                    C.c_uint32(galois_elt), arr(dsts), hr)
+        return dsts, [hres(x) for x in hr]
+
+    def graph_stats(self):
+        """B200_Context_GraphStatsDebug: first sights, captures, refused captures, replays, evictions, batches without a graph"""
+        out = (u64 * 6)()
+        self.S.call("B200_Context_GraphStatsDebug", self.ctx, out)
+        return np.array(list(out), dtype=np.int64)
+
     def decryptor(self, sk_words):
         sk = vp()
         self.S.call("SecretKey_Create1", C.byref(sk))
