@@ -1249,7 +1249,6 @@ struct LevelFpHost
 
 struct b200_ctx
 {
-    unsigned long long *ntt_timeline = nullptr; // developer aid, see b200_ntt_timeline()
     std::vector<LevelFpHost> fp_levels; // indexed like `levels`; empty tables when the level is not on the FP64 path
     std::unique_ptr<BfvHostContext> host;
     int device = 0;
@@ -1683,17 +1682,6 @@ static int get_job(b200_ctx *ctx, const std::string &key, const std::vector<int>
     return 0;
 }
 
-struct TensorArgs
-{
-    int mode = 0, sa = 0, sb = 0, rows = 0;
-    const u64 *src = nullptr;
-};
-
-#ifndef B200_EMU_HEADER
-// FP64 NTT kernel variant (ntt_fp_body.cuh: NttFpStaticPass VAR); B200_NTT_VAR or b200_debug_ntt_variant() override the default
-static std::atomic<int> g_ntt_stagger{ std::getenv("B200_NTT_STAGGER") ? atoi(std::getenv("B200_NTT_STAGGER")) : 0 };
-static std::atomic<int> g_ntt_var{ std::getenv("B200_NTT_VAR") ? atoi(std::getenv("B200_NTT_VAR")) : B200_NTT_DEFAULT_VAR };
-#endif
 static bool static_fp_ok(b200_ctx *ctx, const JobDesc &jd)
 {
 #ifdef B200_EMU_HEADER
@@ -1715,7 +1703,7 @@ struct NttAlt
 
 template <bool FWD>
 static int launch_ntt(b200_ctx *ctx, const JobDesc &jd, const u64 *src, long long src_stride, u64 *dst, long long dst_stride,
-                      long long items, int reduce_input, cudaStream_t s, const TensorArgs *ta = nullptr, const NttAlt *alt = nullptr)
+                      long long items, int reduce_input, cudaStream_t s, const NttAlt *alt = nullptr)
 {
     if (items == 0 || jd.slots == 0)
         return 0;
@@ -1739,24 +1727,6 @@ static int launch_ntt(b200_ctx *ctx, const JobDesc &jd, const u64 *src, long lon
     job.fprimes = ctx->d_fp_primes;
     job.reduce_input = reduce_input;
     job.items = items;
-    static const int pf = std::getenv("B200_NTT_PREFETCH") ? atoi(std::getenv("B200_NTT_PREFETCH")) : 0;
-    job.prefetch_dist = pf;
-    job.timeline = ctx->ntt_timeline;
-    static const int slot_major = std::getenv("B200_NTT_ITEM_MAJOR") ? 0 : 1;
-    job.slot_major = slot_major;
-#ifndef B200_EMU_HEADER
-    job.stagger = g_ntt_stagger.load(std::memory_order_relaxed);
-#else
-    job.stagger = 0;
-#endif
-    job.sm_count = ctx->sm_count;
-    job.tensor_mode = ta ? ta->mode : 0;
-    job.t_sa = ta ? ta->sa : 0;
-    job.t_sb = ta ? ta->sb : 0;
-    job.t_rows = ta ? ta->rows : 0;
-    job.tsrc = ta ? ta->src : nullptr;
-    if (ta && ta->mode && !static_fp_ok(ctx, jd))
-        return fail(B200_E_LOGIC, "internal: fused tensor source needs the static FP64 NTT kernel");
     job.split = ctx->ntt_split;
     job.npass = ctx->npass;
     for (int i = 0; i < 8; i++)
@@ -1794,48 +1764,21 @@ static int launch_ntt(b200_ctx *ctx, const JobDesc &jd, const u64 *src, long lon
     {
         // n = 8192: 256 threads x 3 CTAs/SM is the throughput configuration; a launch that cannot fill the SMs anyway (the
         // per-handle path: at most 36 polynomials) is latency-bound and finishes sooner with 512 threads per polynomial
-        static const int nt_env = std::getenv("B200_NTT_NT") ? atoi(std::getenv("B200_NTT_NT")) : 0;
-        int var_env = g_ntt_var.load(std::memory_order_relaxed);
-        if (var_env < 0)
-        { // automatic: what measured fastest per size and direction (tools/ntt_ablate.py).  2048 = warp(-group)-private
-          // sub-transforms, +1 = first 512 twiddles in shared memory, +16 = streaming (persistent) kernel
-            if (ctx->logn == 14)
-                var_env = FWD ? 2049 : 2064;
-            else if (ctx->logn == 13)
-                var_env = FWD ? 2048 : 2049;
-            else
-                var_env = 2048;
-        }
-        const int nt13 = nt_env ? nt_env : (blocks <= 2LL * ctx->sm_count ? 512 : 256);
-        const int nt = ctx->logn == 12 ? 256 : ctx->logn == 13 ? (nt13 == 256 ? 256 : 512) : 1024;
-        int var = ta && ta->mode ? (var_env & 1) : var_env; // the fused-tensor copy-in exists in the plain variants only
-        if ((var & 16) && nt == 512)
-            var &= ~16; // the streaming variant exists for the throughput configuration; small launches stay latency-optimised
-        b200_ntt_fp_fn sfn = b200_ntt_fp_kernel(ctx->logn, FWD, nt, var);
-        if (!sfn)
-        {
-            var &= 1;
-            sfn = b200_ntt_fp_kernel(ctx->logn, FWD, nt, var);
-        }
-        if (!sfn)
-        {
-            var = 0;
-            sfn = b200_ntt_fp_kernel(ctx->logn, FWD, nt, 0);
-        }
+        const int nt = ctx->logn == 12 ? 256 : ctx->logn == 13 ? (blocks <= 2LL * ctx->sm_count ? 512 : 256) : 1024;
+        const b200_ntt_fp_fn sfn = b200_ntt_fp_kernel(ctx->logn, FWD, nt);
         if (!sfn)
             return fail(B200_E_LOGIC, "internal: no FP64 NTT kernel for this size");
-        const size_t smem = ctx->ntt_smem + ((var & 1) ? B200_NTT_TWS_ENTRIES * sizeof(double) : 0);
+        const B200NttFpLayout K = b200_ntt_fp_layout(ctx->logn, FWD);
         if (trace_on())
         {
             static char labels[2][128][40];
             const int sl = jd.slots < 128 ? jd.slots : 127;
-            snprintf(labels[FWD ? 1 : 0][sl], sizeof(labels[0][0]), "ntt_fp_kernel<%s> rows/item=%d%s", FWD ? "fwd" : "inv", jd.slots,
-                     job.tensor_mode ? " +tensor" : "");
+            snprintf(labels[FWD ? 1 : 0][sl], sizeof(labels[0][0]), "ntt_fp_kernel<%s> rows/item=%d", FWD ? "fwd" : "inv", jd.slots);
             g_trace_name = labels[FWD ? 1 : 0][sl];
         }
         unsigned grid = (unsigned)blocks;
-        if (var & 16)
-        { // persistent: one CTA per resident slot, each walking its share of the polynomials
+        if (K.persistent)
+        { // one CTA per resident slot, each walking its share of the polynomials
             static std::map<b200_ntt_fp_fn, int> occ;
             static std::mutex occ_mu;
             int per_sm;
@@ -1843,21 +1786,18 @@ static int launch_ntt(b200_ctx *ctx, const JobDesc &jd, const u64 *src, long lon
                 std::lock_guard<std::mutex> lk(occ_mu);
                 auto it = occ.find(sfn);
                 if (it == occ.end())
-                    it = occ.emplace(sfn, b200_ntt_fp_ctas_per_sm(sfn, nt, smem)).first;
+                    it = occ.emplace(sfn, b200_ntt_fp_ctas_per_sm(sfn, nt, K.smem)).first;
                 per_sm = it->second;
             }
             grid = (unsigned)std::min<long long>(blocks, (long long)per_sm * ctx->sm_count);
         }
-        B200_LAUNCH(sfn, grid, nt, smem, s, job);
+        B200_LAUNCH(sfn, grid, nt, K.smem, s, job);
         ctx->launches++;
         CU_TRY(cudaGetLastError());
         return 0;
     }
 #endif
-    static const int mb = std::getenv("B200_NTT_INT_MB") ? atoi(std::getenv("B200_NTT_INT_MB")) : 3;
-    void (*kfn)(const NttJob) = ctx->ntt_threads == 512   ? ntt_kernel<FWD, 512>
-                                : ctx->ntt_threads == 256 ? (mb == 2 ? ntt_kernel<FWD, 256, 2> : mb == 1 ? ntt_kernel<FWD, 256, 1> : ntt_kernel<FWD, 256>)
-                                                          : ntt_kernel<FWD, 64>;
+    void (*kfn)(const NttJob) = ctx->ntt_threads == 512 ? ntt_kernel<FWD, 512> : ctx->ntt_threads == 256 ? ntt_kernel<FWD, 256> : ntt_kernel<FWD, 64>;
     B200_LAUNCH(kfn, (unsigned)blocks, ctx->ntt_threads, ctx->ntt_smem, s, job);
     ctx->launches++;
     CU_TRY(cudaGetLastError());
@@ -2059,10 +1999,8 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
 #ifndef B200_EMU_HEADER
     // (3)-(5) in one kernel for a size-2 x size-2 product on the FP64 static path (mul_cluster.cu): the NTT-form operands and
     // products stay in the shared memory of a 4-CTA cluster.  Taken where the launch fills the GPU (the rule of the 256/512
-    // thread switch in launch_ntt); B200_MUL_CLUSTER=0 selects the separate kernels below, B200_TENSOR_FUSION=1 their fused
-    // inverse copy-in.
-    static const bool want_cluster = !(std::getenv("B200_MUL_CLUSTER") && std::getenv("B200_MUL_CLUSTER")[0] == '0') &&
-                                     !std::getenv("B200_TENSOR_FUSION");
+    // thread switch in launch_ntt); B200_MUL_CLUSTER=0 selects the separate kernels below.
+    static const bool want_cluster = !(std::getenv("B200_MUL_CLUSTER") && std::getenv("B200_MUL_CLUSTER")[0] == '0');
     if (want_cluster && !square && sa == 2 && sb == 2 && L.fp && ctx->mul_clusters > 0 && ctx->logn <= 13 &&
         4LL * R * batch > 2LL * ctx->sm_count)
     {
@@ -2135,11 +2073,10 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
         std::string key = "mulfwd:" + std::to_string(level) + ":" + std::to_string(sa) + ":" + std::to_string(square ? 0 : sb);
         if ((rc = get_job(ctx, key, prime, so, dof, &jd)))
             return rc;
-        if ((rc = launch_ntt<true>(ctx, jd, ext, (long long)P * R * n, ext, (long long)P * R * n, batch, 0, s, nullptr, &alt)))
+        if ((rc = launch_ntt<true>(ctx, jd, ext, (long long)P * R * n, ext, (long long)P * R * n, batch, 0, s, &alt)))
             return rc;
     }
-    // (4) tensor + (5) inverse NTTs.  Optionally (FP64 path) the dyadic products are formed inside the inverse
-    // transform's coalesced copy-in (D never materialised in NTT form); by default a separate tensor kernel runs.
+    // (4) tensor + (5) inverse NTTs
     if (!clustered)
     {
         std::vector<int> rows = row_primes(ctx, level, true), prime;
@@ -2148,34 +2085,18 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
         JobDesc jd;
         if ((rc = dense_job(ctx, "muld:" + std::to_string(level) + ":" + std::to_string(Dn), prime, &jd)))
             return rc;
-        // measured on B200 (round 1): the fused variant is SLOWER (10.9 vs 8.9 ms per 1024 ops) — the extra strided
-        // loads sit on the transform's latency-critical copy-in — so it stays opt-in (B200_TENSOR_FUSION=1)
-        static const bool want_fuse = std::getenv("B200_TENSOR_FUSION") != nullptr;
-        const bool fuse = want_fuse && L.fp && static_fp_ok(ctx, jd);
-        TensorArgs ta;
-        if (fuse)
+        if (L.fp && (square || (sa == 2 && sb == 2)))
         {
-            ta.mode = square ? 2 : 1;
-            ta.sa = sa;
-            ta.sb = sb;
-            ta.rows = R;
-            ta.src = ext;
+            const long long total = batch * R * (n >> 1);
+            B200_LAUNCH(tensor_kernel_v2, blocks_for(total, EB), EB, 0, s, L, ext, D, n, total, square ? 1 : 0);
         }
         else
         {
-            if (L.fp && (square || (sa == 2 && sb == 2)))
-            {
-                const long long total = batch * R * (n >> 1);
-                B200_LAUNCH(tensor_kernel_v2, blocks_for(total, EB), EB, 0, s, L, ext, D, n, total, square ? 1 : 0);
-            }
-            else
-            {
-                const long long total = batch * R * n;
-                B200_LAUNCH(tensor_kernel, blocks_for(total, EB), EB, 0, s, L, ext, sa, sb, D, n, total, square ? 1 : 0);
-            }
-            ctx->launches++;
+            const long long total = batch * R * n;
+            B200_LAUNCH(tensor_kernel, blocks_for(total, EB), EB, 0, s, L, ext, sa, sb, D, n, total, square ? 1 : 0);
         }
-        if ((rc = launch_ntt<false>(ctx, jd, D, (long long)Dn * R * n, D, (long long)Dn * R * n, batch, 0, s, fuse ? &ta : nullptr)))
+        ctx->launches++;
+        if ((rc = launch_ntt<false>(ctx, jd, D, (long long)Dn * R * n, D, (long long)Dn * R * n, batch, 0, s)))
             return rc;
     }
     // (6)-(8) scale
@@ -2623,14 +2544,8 @@ int b200_ctx_create(uint64_t n, const uint64_t *coeff_modulus, uint64_t count, u
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<false, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
 #ifndef B200_EMU_HEADER
-    CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
-    CU_TRY(cudaFuncSetAttribute(ntt_kernel<false, 256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
-    CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 256, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
-    CU_TRY(cudaFuncSetAttribute(ntt_kernel<false, 256, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 256>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<false, 256>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 256, 2>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    CU_TRY(cudaFuncSetAttribute(ntt_kernel<false, 256, 2>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
 #endif
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<true, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
     CU_TRY(cudaFuncSetAttribute(ntt_kernel<false, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)prop.sharedMemPerBlockOptin));
@@ -2877,47 +2792,20 @@ int b200_stream_synchronize(b200_ctx *ctx, void *stream)
     return 0;
 }
 
-// developer aid: attach a device buffer of 8 u64 per CTA that the NEXT static NTT launches fill with
-// {smid, t_start, t_after_each_pass (<=5), t_end} (globaltimer ns); pass nullptr to detach
-int b200_debug_ntt_stagger(int cycles)
+int b200_debug_ntt_ctas_per_sm(int logn, int forward, int threads)
 {
 #ifndef B200_EMU_HEADER
-    return g_ntt_stagger.exchange(cycles);
-#else
-    (void)cycles;
-    return 0;
-#endif
-}
-int b200_debug_ntt_variant(int variant)
-{
-#ifndef B200_EMU_HEADER
-    return g_ntt_var.exchange(variant);
-#else
-    (void)variant;
-    return 0;
-#endif
-}
-int b200_debug_ntt_ctas_per_sm(int logn, int forward, int threads, int variant)
-{
-#ifndef B200_EMU_HEADER
-    // the query launch_ntt makes for the grid of the persistent variant (same kernel, same dynamic shared memory)
-    b200_ntt_fp_fn sfn = b200_ntt_fp_kernel(logn, forward != 0, threads, variant);
+    // the query launch_ntt makes for the grid of the persistent kernel (same kernel, same dynamic shared memory)
+    const b200_ntt_fp_fn sfn = b200_ntt_fp_kernel(logn, forward != 0, threads);
     if (!sfn)
-        return fail(B200_E_INVALID, "no FP64 NTT kernel for this (size, direction, CTA width, variant)");
-    const size_t smem = (size_t)ntt_smem_words(1 << logn) * sizeof(u64) + ((variant & 1) ? B200_NTT_TWS_ENTRIES * sizeof(double) : 0);
-    return b200_ntt_fp_ctas_per_sm(sfn, threads, smem);
+        return fail(B200_E_INVALID, "no FP64 NTT kernel for this (size, direction, CTA width)");
+    return b200_ntt_fp_ctas_per_sm(sfn, threads, b200_ntt_fp_layout(logn, forward != 0).smem);
 #else
     (void)logn;
     (void)forward;
     (void)threads;
-    (void)variant;
     return fail(B200_E_INVALID, "the emulation build has no FP64 NTT kernels");
 #endif
-}
-void b200_ntt_timeline(b200_ctx *ctx, unsigned long long *device_buffer)
-{
-    if (ctx)
-        ctx->ntt_timeline = device_buffer;
 }
 
 void b200_trace_dump(void)

@@ -3,9 +3,9 @@
 //
 // The product D = (a0 + a1 y)(b0 + b1 y) of residue row r needs the four NTT-form rows a0, a1, b0, b1 at once: 4 x 64 KiB at
 // n = 8192, more than one CTA's shared memory but within a 4-CTA thread-block cluster's.  CTA c of the cluster transforms
-// operand c in its own shared memory (NttFpStaticPass, VAR & 4096: no copy-out), the dyadic step reads the operands of each
+// operand c in its own shared memory (NttFpStaticPass with the HANDOFF option: no copy-out), the dyadic step reads the operands of each
 // coefficient through distributed shared memory and writes D0, D1, D2 into the buffers of CTAs 0, 1, 2, which transform them
-// back from there (VAR & 4096: no copy-in) and write D in coefficient form.  The separate path moves the same rows through
+// back from there (HANDOFF: no copy-in) and write D in coefficient form.  The separate path moves the same rows through
 // HBM three more times (forward write, tensor read + write, inverse read: 126 of its 264 rows per item at k = 4, |Bsk| = 5).
 //
 // Every intermediate word equals the separate path's: the operands are brought to canonical form before the products (the
@@ -26,8 +26,9 @@ namespace
 {
 constexpr int NT = 256;        // threads per CTA: the n = 8192 throughput configuration (3 CTAs per SM)
 constexpr int CLUSTER = 4;     // CTAs per cluster: operands a0, a1, b0, b1
-constexpr int FWD_VAR = 2048 | 4096;     // warp-private passes, result stays in shared memory
-constexpr int INV_VAR = 2048 | 1 | 4096; // + first 512 twiddles in shared memory, input already in shared memory
+using FwdOpt = NttFpOpt<false, false, true>;            // result stays in shared memory
+using GalOpt = NttFpOpt<false, false, true, true>;      // the same, first pass gathers sigma_g(src)
+using InvOpt = NttFpOpt<true, false, true>;             // first twiddles in shared memory, input already in shared memory
 
 template <int LOGN>
 constexpr size_t smem_bytes()
@@ -77,7 +78,7 @@ __global__ void __launch_bounds__(NT, 3) mul_cluster_kernel(const NttJob job, co
     const NttPrime PI_ = job.primes[job.slot_prime[w.r]];
     // operand c (a0, a1, b0, b1): q rows straight from the ciphertexts, Bsk rows from the lifted rows
     const u64 *src = w.r < k ? (w.c < 2 ? a : b) + ((w.item * 2 + (w.c & 1)) * k + w.r) * N : ext + ((w.item * CLUSTER + w.c) * R + w.r) * N;
-    NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR>::run(job, PF, PI_, src, nullptr, smd, tid, w.item, w.r);
+    NttFpStaticPass<LOGN, NT, true, 0, FwdOpt>::run(job, PF, PI_, src, nullptr, smd, tid);
     cluster_sync(); // all four operands transformed
     w = place(job);
 
@@ -127,7 +128,7 @@ __global__ void __launch_bounds__(NT, 3) mul_cluster_kernel(const NttJob job, co
         return;
     u64 *dst = D + ((w.item * 3 + w.c) * R + w.r) * N;
     const NttPrimeFp PFi = job.fprimes[job.slot_prime[w.r]]; // (loaded again: nothing of the forward phase stays live)
-    NttFpStaticPass<LOGN, NT, false, 0, INV_VAR>::run(job, PFi, job.primes[job.slot_prime[w.r]], nullptr, dst, smd, tid, w.item, w.r);
+    NttFpStaticPass<LOGN, NT, false, 0, InvOpt>::run(job, PFi, job.primes[job.slot_prime[w.r]], nullptr, dst, smd, tid);
 }
 
 // ks_cluster_kernel's place: rank J in the cluster (digit J), key residue I in [0, k] (k: the special prime), item.  Items
@@ -167,14 +168,13 @@ __device__ __forceinline__ void ks_cluster_body(const NttJob &job, const u64 *d,
         // digit J of the target, reduced mod p_I by the first pass (job.reduce_input)
         const u64 *dj = MULTI ? nullptr : d + w.item * d_stride + (long long)w.J * N;
         if constexpr (MULTI)
-            NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR | 8192>::run(job, PF, PI_, tab[w.item].ct + (long long)(k + w.J) * N, nullptr, smd,
-                                                                    tid, w.item, w.I, nullptr, tab[w.item].ginv,
-                                                                    job.primes[job.slot_prime[w.J]].p);
+            NttFpStaticPass<LOGN, NT, true, 0, GalOpt>::run(job, PF, PI_, tab[w.item].ct + (long long)(k + w.J) * N, nullptr, smd, tid,
+                                                            nullptr, tab[w.item].ginv, job.primes[job.slot_prime[w.J]].p);
         else if constexpr (GAL)
-            NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR | 8192>::run(job, PF, PI_, dj, nullptr, smd, tid, w.item, w.I, nullptr, ginv,
-                                                                    job.primes[job.slot_prime[w.J]].p);
+            NttFpStaticPass<LOGN, NT, true, 0, GalOpt>::run(job, PF, PI_, dj, nullptr, smd, tid, nullptr, ginv,
+                                                            job.primes[job.slot_prime[w.J]].p);
         else
-            NttFpStaticPass<LOGN, NT, true, 0, FWD_VAR>::run(job, PF, PI_, dj, nullptr, smd, tid, w.item, w.I);
+            NttFpStaticPass<LOGN, NT, true, 0, FwdOpt>::run(job, PF, PI_, dj, nullptr, smd, tid);
     }
     cluster_sync(); // all k digits transformed
     w = ks_place(k);
@@ -249,7 +249,7 @@ __device__ __forceinline__ void ks_cluster_body(const NttJob &job, const u64 *d,
         return;
     u64 *dst = ks2 + ((w.item * 2 + w.J) * (k + 1) + w.I) * N;
     const int pi = job.slot_prime[w.I]; // (loaded again: nothing of the inner product stays live)
-    NttFpStaticPass<LOGN, NT, false, 0, INV_VAR>::run(job, job.fprimes[pi], job.primes[pi], nullptr, dst, smd, tid, w.item, w.I);
+    NttFpStaticPass<LOGN, NT, false, 0, InvOpt>::run(job, job.fprimes[pi], job.primes[pi], nullptr, dst, smd, tid);
 }
 
 template <int LOGN>

@@ -62,18 +62,6 @@ struct NttJob
     const NttPrimeFp *fprimes; // FP64 fast-path descriptors, same indexing as primes[]
     int reduce_input;          // 1: inputs are arbitrary 64-bit words -> Barrett to [0,p) on load
     long long items;           // number of items in this launch
-    int prefetch_dist;         // >0: each CTA prefetches (L2) the input of CTA blockIdx + prefetch_dist
-    unsigned long long *timeline; // developer aid (B200_NTT_TIMELINE): per CTA {smid, t_start, t_after_pass_1..4, t_end} in ns
-    int slot_major;            // block order (static FP kernel): 1 = all items of slot 0, then slot 1, ...
-    int stagger;               // streaming FP kernel: CTA of resident slot s (blockIdx / #SMs) starts s * stagger clock cycles late,
-                               // so that the CTAs sharing an SM are in different phases (one moving data while the others compute)
-    int sm_count;
-    // fused tensor source (FP64 static inverse kernel only): instead of reading `src`, slot (m, row) computes
-    // D_m[row] = sum_{r+s=m} A_r[row] * B_s[row] on the fly from the NTT-form operands at `tsrc`
-    // ([item][sa+sb (or sa when squaring)][trows][n]); 0 = off, 1 = product, 2 = square of a size-2 ciphertext
-    int tensor_mode;
-    int t_sa, t_sb, t_rows;
-    const u64 *tsrc;
     int split;                 // 1: n is too large for one CTA: each CTA transforms one HALF (size n/2) as a sub-transform;
                                //    the remaining butterfly stage over the whole polynomial runs in ntt_outer_kernel
     int npass;                 // forward pass schedule (host: ntt_schedule); inverse runs it mirrored

@@ -139,18 +139,16 @@ B200_HD double fp_load_tw(const double *__restrict__ tw, int idx)
 // All R-1 twiddles of a radix-2^L group, loaded up front so that their (L2) latency is paid once per group and
 // overlaps the data loads.  Slot order: forward stage l, sub-group grp -> (2^l - 1) + grp;
 // inverse stage l, sub-group grp -> R - (R >> l) + grp  (the TW16 tables use the same slot order).
-// TWSRC: 0 = read-only global path (__ldg), 1 = `tw` points at the CTA's shared-memory copy of the table's first 512
-// entries (plain load), 2 = developer ablation (no load at all: a constant stands in; results are meaningless)
-template <int TWSRC>
-B200_HD double fp_load_tw_src(const double *__restrict__ tw, int idx, const NttPrimeFp &P)
+// STW: `tw` points at the CTA's shared-memory copy of the table's first B200_NTT_TWS_ENTRIES entries (plain load) instead
+// of the table in global memory (read-only path, __ldg)
+template <bool STW>
+B200_HD double fp_load_tw_src(const double *__restrict__ tw, int idx)
 {
-    if (TWSRC == 2)
-        return B200_DADD(P.inv_n[0], (double)(idx & 7));
-    if (TWSRC == 1)
+    if (STW)
         return tw[idx];
     return fp_load_tw(tw, idx);
 }
-template <int L, bool FWD, bool TW16, int TWSRC = 0>
+template <int L, bool FWD, bool TW16, bool STW = false>
 B200_HD void fp_load_group_tw(double (&tws)[(1 << L) - 1], const double *__restrict__ tw, int g, int i, int logs, int logn, int M,
                               int n16, const NttPrimeFp &P, bool last_inv)
 {
@@ -165,7 +163,7 @@ B200_HD void fp_load_group_tw(double (&tws)[(1 << L) - 1], const double *__restr
             for (int grp = 0; grp < (1 << l); grp++)
             {
                 const int slot = (1 << l) - 1 + grp;
-                tws[slot] = fp_load_tw_src<TWSRC>(tw, TW16 ? slot * n16 + g : tw_base + grp, P);
+                tws[slot] = fp_load_tw_src<STW>(tw, TW16 ? slot * n16 + g : tw_base + grp);
             }
         }
         else
@@ -179,22 +177,14 @@ B200_HD void fp_load_group_tw(double (&tws)[(1 << L) - 1], const double *__restr
                 if (last_inv && l == L - 1)
                     tws[slot] = P.inv_n_w[0]; // final stage of the whole inverse: twiddle pre-multiplied by n^-1
                 else
-                    tws[slot] = fp_load_tw_src<TWSRC>(tw, TW16 ? slot * n16 + g : tw_base + grp, P);
+                    tws[slot] = fp_load_tw_src<STW>(tw, TW16 ? slot * n16 + g : tw_base + grp);
             }
         }
     }
 }
 
 // one butterfly stage `l` of a radix-2^L group (compile-time stage index so everything stays in registers)
-// ABL bit 0 (developer ablation): the modular product is replaced by one DMUL (results are meaningless)
-template <int ABL>
-B200_HD double fp_mulmod_abl(double a, double b, double p, double pinv)
-{
-    if (ABL & 1)
-        return B200_DMUL(a, b);
-    return fp_mulmod2(a, b, p, pinv);
-}
-template <int L, int l, bool FWD, int ABL = 0>
+template <int L, int l, bool FWD>
 B200_HD void fp_stage(double (&x)[1 << L], const double (&tws)[(1 << L) - 1], const NttPrimeFp &P, bool last_inv)
 {
     constexpr int R = 1 << L;
@@ -210,7 +200,7 @@ B200_HD void fp_stage(double (&x)[1 << L], const double (&tws)[(1 << L) - 1], co
             for (int jj = 0; jj < half; jj++)
             {
                 const int j = grp * 2 * half + jj;
-                const double T = fp_mulmod_abl<ABL>(x[j + half], w, p, pinv);
+                const double T = fp_mulmod2(x[j + half], w, p, pinv);
                 const double X = x[j];
                 x[j] = B200_DADD(X, T);
                 x[j + half] = B200_DADD(X, -T);
@@ -231,7 +221,7 @@ B200_HD void fp_stage(double (&x)[1 << L], const double (&tws)[(1 << L) - 1], co
                 const int j = grp * 2 * half + jj;
                 const double X = x[j], Y = x[j + half];
                 const double U = B200_DADD(X, Y);
-                x[j + half] = fp_mulmod_abl<ABL>(B200_DADD(X, -Y), w, p, pinv);
+                x[j + half] = fp_mulmod2(B200_DADD(X, -Y), w, p, pinv);
                 x[j] = fold ? fp_mulmod2(U, P.inv_n[0], p, pinv) : U;
             }
         }
@@ -253,13 +243,13 @@ B200_HD int fp_elem_index(int pbase, int base, int j, int logs)
 template <int L, bool FWD, bool SRC_GLOBAL, bool DST_GLOBAL, bool TW16 = false, bool RENORM = true, bool REDUCE = true, bool PRELOADED = false,
           bool RAW_IN = false /* shared memory holds the raw input words (landed by cp.async): convert on read */,
           bool TW_PRE = false /* the group's twiddles were prefetched by the caller (twpre) */,
-          int TWSRC = 0 /* fp_load_tw_src */, int ABL = 0 /* developer ablations: 1 cheap product, 2 no global loads, 4 no global stores */,
+          bool STW = false /* fp_load_tw_src */,
           bool REFILL = false /* streaming kernel, last inverse pass: once this group's inputs have been consumed, the NEXT
                                  polynomial's words for the same slots are requested (cp.async) from `refill` */>
 B200_HD void ntt_fp_group(double *sm, const u64 *__restrict__ gsrc, u64 *__restrict__ gdst, int g, int logs, int logn, int M,
                           const NttPrimeFp &P, bool renorm, bool last_inv, bool reduce_input, u64 pint, u64 ratio1,
                           const u64 *pre = nullptr /* PRELOADED: the group's 2^L raw input words, already in registers */,
-                          const double *twpre = nullptr, const double *stw = nullptr /* TWSRC == 1: shared-memory table */,
+                          const double *twpre = nullptr, const double *stw = nullptr /* STW: shared-memory table */,
                           const u64 *refill = nullptr)
 {
     constexpr int R = 1 << L;
@@ -269,7 +259,7 @@ B200_HD void ntt_fp_group(double *sm, const u64 *__restrict__ gsrc, u64 *__restr
     const int base = (i << (logs + L)) + o;
     const int pbase = ntt_pad(base);
     const double p = P.p;
-    const double *__restrict__ tw = TWSRC == 1 ? stw : TW16 ? (FWD ? P.fwd16 : P.inv16) : (FWD ? P.fwd : P.inv);
+    const double *__restrict__ tw = STW ? stw : TW16 ? (FWD ? P.fwd16 : P.inv16) : (FWD ? P.fwd : P.inv);
     const int n16 = 1 << (logn - 4); // groups of the radix-16 pass (TW16 layout: [slot][group])
     double tws[R - 1];
     if (TW_PRE)
@@ -279,14 +269,14 @@ B200_HD void ntt_fp_group(double *sm, const u64 *__restrict__ gsrc, u64 *__restr
             tws[j] = twpre[j];
     }
     else
-        fp_load_group_tw<L, FWD, TW16, TWSRC>(tws, tw, g, i, logs, logn, M, n16, P, last_inv);
+        fp_load_group_tw<L, FWD, TW16, STW>(tws, tw, g, i, logs, logn, M, n16, P, last_inv);
     double x[R];
 #pragma unroll
     for (int j = 0; j < R; j++)
     {
         if (SRC_GLOBAL)
         {
-            u64 v = PRELOADED ? pre[j] : (ABL & 2) ? (u64)(base + j) : gsrc[base + (j << logs)];
+            u64 v = PRELOADED ? pre[j] : gsrc[base + (j << logs)];
             if (REDUCE && reduce_input)
                 v = barrett64(v, pint, ratio1);
             x[j] = fp_from_u64(v);
@@ -312,13 +302,13 @@ B200_HD void ntt_fp_group(double *sm, const u64 *__restrict__ gsrc, u64 *__restr
         if (RENORM && renorm)
             x[j] = fp_renorm_x(x[j], p, P.pinv);
     }
-    fp_stage<L, 0, FWD, ABL>(x, tws, P, last_inv);
+    fp_stage<L, 0, FWD>(x, tws, P, last_inv);
     if constexpr (L > 1)
-        fp_stage<L, 1, FWD, ABL>(x, tws, P, last_inv);
+        fp_stage<L, 1, FWD>(x, tws, P, last_inv);
     if constexpr (L > 2)
-        fp_stage<L, 2, FWD, ABL>(x, tws, P, last_inv);
+        fp_stage<L, 2, FWD>(x, tws, P, last_inv);
     if constexpr (L > 3)
-        fp_stage<L, 3, FWD, ABL>(x, tws, P, last_inv);
+        fp_stage<L, 3, FWD>(x, tws, P, last_inv);
 #if defined(__CUDA_ARCH__)
     if (REFILL && !SRC_GLOBAL && refill)
     {
@@ -334,21 +324,8 @@ B200_HD void ntt_fp_group(double *sm, const u64 *__restrict__ gsrc, u64 *__restr
 #pragma unroll
     for (int j = 0; j < R; j++)
     {
-        if (DST_GLOBAL && (ABL & 4))
-        {
-            const u64 v = fp_to_canonical<true>(x[j], p, P.pinv);
-            if (v == 0xFFFFFFFFFFFFFFFFULL) // never: keeps the value live without the store traffic
-                gdst[base + (j << logs)] = v;
-        }
-        else if (DST_GLOBAL)
-        {
-#if defined(__CUDA_ARCH__)
-            if (ABL & 8)
-                __stcs(gdst + base + (j << logs), fp_to_canonical<true>(x[j], p, P.pinv));
-            else
-#endif
-                gdst[base + (j << logs)] = fp_to_canonical<true>(x[j], p, P.pinv);
-        }
+        if (DST_GLOBAL)
+            gdst[base + (j << logs)] = fp_to_canonical<true>(x[j], p, P.pinv);
         else
             sm[fp_elem_index(pbase, base, j, logs)] = x[j];
     }
@@ -464,20 +441,29 @@ template <int LOGN, int PI> struct NttSchedDone // stages completed before forwa
 };
 template <int LOGN> struct NttSchedDone<LOGN, 0> { static constexpr int value = 0; };
 
-// VAR (bit mask): 1 = the table's first 512 twiddles (every stage whose butterflies span >= n/256 points) are copied into
-// shared memory once per CTA and read from there (short latency, no L2 round trip per group); 2 / 4 / 8 = developer
-// ablations for tools/ntt_ablate.py (no twiddle loads / one-DMUL products / no global traffic): results are meaningless,
-// they only measure what each component costs.
-// VAR & 8192 (forward only): the first pass reads sigma_g(src) instead of src, for the Galois automorphism X -> X^g of a
-// coefficient-form row mod q: destination word e is source word i = e g^-1 mod 2n, negated mod q (gal_q) where i >= n.  `gal`
-// is g^-1 mod 2n.  The negation happens mod q, before job.reduce_input reduces the word mod the transform's prime.
+// Compile-time options of a transform; every combination in use is a shipped kernel (ntt_fp_kernels.cu, mul_cluster.cu).
+//   SMEM_TW  the table's first B200_NTT_TWS_ENTRIES twiddles (every stage whose butterflies span >= n/256 points) are copied
+//            into shared memory once per CTA and read from there (short latency, no L2 round trip per group).
+//   STREAM   (inverse) persistent kernel: the polynomial's raw words are ALREADY on their way into shared memory when the
+//            transform starts (requested during the previous polynomial's last pass, into slots that pass had finished with),
+//            and the last pass requests the next polynomial's words (`nsrc`) the same way.
+//   HANDOFF  the polynomial stays in shared memory at the hand-off to / from the fused dyadic step (mul_cluster.cu): the
+//            forward transform leaves its lazy result there (no copy-out), the inverse finds canonical values there (no copy-in).
+//   GATHER   (forward) the first pass reads sigma_g(src) instead of src, for the Galois automorphism X -> X^g of a
+//            coefficient-form row mod q: destination word e is source word i = e g^-1 mod 2n, negated mod q (gal_q) where
+//            i >= n.  `gal` is g^-1 mod 2n.  The negation happens mod q, before job.reduce_input reduces the word mod the
+//            transform's prime.
+template <bool SMEM_TW_, bool STREAM_ = false, bool HANDOFF_ = false, bool GATHER_ = false>
+struct NttFpOpt
+{
+    static constexpr bool SMEM_TW = SMEM_TW_, STREAM = STREAM_, HANDOFF = HANDOFF_, GATHER = GATHER_;
+};
 #define B200_NTT_TWS_ENTRIES 512
-template <int LOGN, int NT, bool FWD, int STEP /*0..NP-1 in execution order*/, int VAR = 0>
+template <int LOGN, int NT, bool FWD, int STEP /*0..NP-1 in execution order*/, class OPT>
 struct NttFpStaticPass
 {
     static __device__ __forceinline__ void run(const NttJob &job, const NttPrimeFp &P, const NttPrime &PI_, const u64 *src, u64 *dst,
-                                               double *smd, int tid, long long item, int slot, const u64 *nsrc = nullptr,
-                                               unsigned gal = 0, u64 gal_q = 0)
+                                               double *smd, int tid, const u64 *nsrc = nullptr, unsigned gal = 0, u64 gal_q = 0)
     {
 #if defined(__CUDA_ARCH__)
         constexpr int N = 1 << LOGN;
@@ -487,24 +473,17 @@ struct NttFpStaticPass
         constexpr int DONE = NttSchedDone<LOGN, PIDX>::value;  // forward stages before this pass
         constexpr int LOGS = LOGN - DONE - L;                  // log2 sub-stride (same for the mirrored inverse pass)
         constexpr int M = 1 << DONE;
+        constexpr bool EDGE_IN = STEP == 0, EDGE_OUT = STEP == NP - 1;
+        constexpr bool STREAM = OPT::STREAM;
+        static_assert(!STREAM || !FWD, "streaming input is an inverse option");
+        static_assert(!OPT::GATHER || FWD, "the Galois gather is a forward option");
         // Direct global I/O only where consecutive lanes touch consecutive words (large sub-stride).  The
         // sub-stride-1 pass would make every lane touch its own 128-byte line (32 L1 wavefronts per request), so
-        // its global side is staged through shared memory with coalesced copies instead.
-        constexpr bool EDGE_IN = STEP == 0, EDGE_OUT = STEP == NP - 1;
-#ifndef B200_NTT_TW_PREFETCH
-#define B200_NTT_TW_PREFETCH 1
-#endif
-#ifndef B200_NTT_DIRECT_IN
-#define B200_NTT_DIRECT_IN 1
-#endif
-        // Direct global I/O only where consecutive lanes touch consecutive words (large sub-stride).  Staging the forward
-        // input through cp.async instead (B200_NTT_DIRECT_IN=0) measures the same within noise (0.72 vs 0.71 ms for
-        // 16384 polynomials): the per-CTA timeline (tools/ntt_timeline.py) shows the copy-in itself takes only 2.6 us of
-        // a CTA's 18.4 us; the kernel is co-limited by the FP64 pipe (52 %) and the shared-memory pipe (55-58 %).
-        // VAR & 16: streaming (persistent) kernel — the polynomial's raw words are ALREADY on their way into shared memory when a
-        // pass sequence starts (requested during the previous polynomial's last pass, into slots that pass had finished with)
-        constexpr bool STREAM = (VAR & 16) != 0;
-        // VAR & 2048: warp-private sub-transforms.  After the first forward pass (radix 2^L0) the polynomial falls apart into 2^L0
+        // its global side is staged through shared memory with coalesced copies instead.  Staging the forward input
+        // through cp.async as well measured the same within noise (0.72 vs 0.71 ms for 16384 polynomials): the copy-in
+        // itself takes only 2.6 us of a CTA's 18.4 us; the kernel is co-limited by the FP64 pipe (52 %) and the
+        // shared-memory pipe (55-58 %).
+        // Warp-private sub-transforms.  After the first forward pass (radix 2^L0) the polynomial falls apart into 2^L0
         // independent blocks of N >> L0 points; with the blocks divided evenly among the warps each warp owns its block(s) for the remaining passes, so
         // those passes (and the write-out of the block) need only __syncwarp — one block-wide barrier per polynomial instead of
         // four — and the block's early-pass twiddles are warp-uniform.  The inverse mirrors it (warp-private until the last pass).
@@ -513,21 +492,18 @@ struct NttFpStaticPass
         constexpr int WP_BLOCKS = 1 << NttSchedL<LOGN, 0>::value, WP_WARPS = NT / 32;
         constexpr int WP_TG = WP_WARPS > WP_BLOCKS ? 32 * (WP_WARPS / WP_BLOCKS) : 32; // threads of one group
         constexpr int WP_NG = NT / WP_TG;                                               // groups in the CTA (<= 15 named barriers)
-        constexpr bool WP = (VAR & 2048) != 0 && (WP_BLOCKS % WP_NG) == 0 && WP_NG <= 15 && !(STREAM && FWD);
-        constexpr bool WPSTEP = WP && (FWD ? STEP >= 1 : STEP + 1 < NP); // this pass runs group-private
-        const int wlane = tid % WP_TG, wwarp = tid / WP_TG;                // position inside the group, group index
+        static_assert(WP_BLOCKS % WP_NG == 0 && WP_NG <= 15, "every group owns whole blocks and has a named barrier");
+        constexpr bool WPSTEP = FWD ? STEP >= 1 : STEP + 1 < NP; // this pass runs group-private
+        const int wlane = tid % WP_TG, wwarp = tid / WP_TG;      // position inside the group, group index
         auto wp_sync = [&]() {
             if constexpr (WP_TG == 32)
                 __syncwarp();
             else
                 asm volatile("bar.sync %0, %1;" ::"r"(1 + wwarp), "r"(WP_TG) : "memory");
         };
-        // VAR & 4096: the polynomial stays in shared memory at the hand-off to / from the fused dyadic step (mul_cluster.cu): the
-        // forward transform leaves its lazy result there (no copy-out), the inverse finds canonical values there (no copy-in)
-        constexpr bool KEEP_OUT = (VAR & 4096) != 0 && FWD, SMEM_IN = (VAR & 4096) != 0 && !FWD;
-        constexpr bool SG = EDGE_IN && LOGS >= 5 && B200_NTT_DIRECT_IN && !STREAM && !SMEM_IN,
-                       DG = EDGE_OUT && LOGS >= 5 && !(VAR & 128) && !KEEP_OUT; // 128: always stage the output
-        constexpr bool GATHER = (VAR & 8192) != 0 && FWD && EDGE_IN;
+        constexpr bool KEEP_OUT = OPT::HANDOFF && FWD, SMEM_IN = OPT::HANDOFF && !FWD;
+        constexpr bool SG = EDGE_IN && LOGS >= 5 && !STREAM && !SMEM_IN, DG = EDGE_OUT && LOGS >= 5 && !KEEP_OUT;
+        constexpr bool GATHER = OPT::GATHER && EDGE_IN;
         static_assert(!GATHER || SG, "the Galois gather reads the first pass's words straight from global memory");
         auto gather_ld = [&](int e) -> u64 {
             const unsigned i = ((unsigned)e * gal) & (2u * N - 1u);
@@ -535,10 +511,9 @@ struct NttFpStaticPass
             return i < (unsigned)N ? x : (x ? gal_q - x : 0);
         };
         constexpr bool TW16 = (L == 4 && LOGS == 0);
-        constexpr int TWSRC = (VAR & 2) ? 2 : ((VAR & 1) && !TW16 && (1 << (DONE + L)) <= B200_NTT_TWS_ENTRIES) ? 1 : 0;
-        constexpr int ABL = ((VAR & 4) ? 1 : 0) | ((VAR & (8 | 32)) ? 2 : 0) | ((VAR & (8 | 64)) ? 4 : 0) | ((VAR & 512) ? 8 : 0); // 32 / 64: loads / stores only; 512: streaming (evict-first) hints
-        double *stw = smd + ntt_smem_words(N); // VAR & 1: B200_NTT_TWS_ENTRIES doubles behind the polynomial
-        if (STEP == 0 && (VAR & 1))
+        constexpr bool STW = OPT::SMEM_TW && !TW16 && (1 << (DONE + L)) <= B200_NTT_TWS_ENTRIES;
+        double *stw = smd + ntt_smem_words(N); // SMEM_TW: B200_NTT_TWS_ENTRIES doubles behind the polynomial
+        if (STEP == 0 && OPT::SMEM_TW)
         {
             const double *__restrict__ twg = FWD ? P.fwd : P.inv;
             for (int e = tid; e < B200_NTT_TWS_ENTRIES; e += NT)
@@ -548,136 +523,44 @@ struct NttFpStaticPass
         }
         constexpr int NGROUPS = N >> L;
         constexpr int ITERS = (NGROUPS + NT - 1) / NT;
-        const bool rn = (((FWD ? P.renorm_fwd : P.renorm_inv) >> STEP) & 1) || (!FWD && STEP == 0 && job.tensor_mode);
+        const bool rn = ((FWD ? P.renorm_fwd : P.renorm_inv) >> STEP) & 1;
         const bool red = EDGE_IN && job.reduce_input != 0;
-        const int ptid = ntt_pad(tid);              // NT is a multiple of 16: pad(tid + it*NT) = pad(tid) + it*(NT + NT/16)
-        constexpr int PNT = NT + (NT >> 4);
         if constexpr (EDGE_IN && SMEM_IN)
             __syncthreads(); // the whole CTA's twiddle copy above is complete (the first pass may span other warps' values)
-        else if (EDGE_IN && !SG)
-        { // coalesced copy-in: u64 -> double
-            if (!FWD && job.tensor_mode)
+        else if constexpr (EDGE_IN && !SG)
+        {
+            // staged copy-in of the inverse (its first pass has sub-stride 1): asynchronous copies (LDGSTS) hold no registers,
+            // so all requests of a thread are in flight at once; the words land raw and the first pass converts them when it
+            // reads (RAW_IN)
+            static_assert(!FWD, "the forward transform's first pass reads global memory directly");
+            if constexpr (STREAM)
             {
-                // fused BEHZ step (4): this slot is (m, row); operands are canonical NTT-form words
-                const int R = job.t_rows;
-                const int m = slot / R, row = slot - m * R;
-                const int np_ = job.tensor_mode == 2 ? job.t_sa : job.t_sa + job.t_sb;
-                const long long ps = (long long)R * N; // polynomial stride inside an item
-                const u64 *A = job.tsrc + ((long long)item * np_ * R + row) * N;
-                const u64 *B = job.tensor_mode == 2 ? A : A + (long long)job.t_sa * ps;
-#pragma unroll
-                for (int it = 0; it < N / NT; it++)
-                {
-                    const int e = tid + it * NT;
-                    double acc = 0.0;
-                    if (job.tensor_mode == 2)
-                    {
-                        const double a0 = fp_from_u64(A[e]), a1 = fp_from_u64(A[ps + e]);
-                        if (m == 0)
-                            acc = fp_mulmod2(a0, a0, P.p, P.pinv);
-                        else if (m == 1)
-                        {
-                            acc = fp_mulmod2(a0, a1, P.p, P.pinv);
-                            acc = B200_DADD(acc, acc);
-                        }
-                        else
-                            acc = fp_mulmod2(a1, a1, P.p, P.pinv);
-                    }
-                    else
-                    {
-                        for (int r = 0; r < job.t_sa; r++)
-                        {
-                            const int s = m - r;
-                            if (s >= 0 && s < job.t_sb)
-                                acc = B200_DADD(acc, fp_mulmod2(fp_from_u64(A[r * ps + e]), fp_from_u64(B[s * ps + e]), P.p, P.pinv));
-                        }
-                    }
-                    smd[ptid + it * PNT] = acc; // lazy, |acc| < 4p: the first pass renormalises if its bound needs it
-                }
-            }
-            else if (STREAM)
                 asm volatile("cp.async.wait_all;" ::: "memory"); // requested by the kernel prologue / the previous polynomial's last pass
-            else
-            {
-                // asynchronous copy (LDGSTS): no registers are held, so all N/NT requests of a thread are in flight at
-                // once; the words land raw and the first pass converts them when it reads (RAW_IN)
-                const unsigned sbase = (unsigned)__cvta_generic_to_shared(smd + ptid);
-                if (ABL & 2)
-                {
-#pragma unroll
-                    for (int it = 0; it < N / NT; it++)
-                        smd[ptid + it * PNT] = __longlong_as_double((long long)(tid + it * NT));
-                }
-                else if (WP && !FWD && !STREAM)
-                { // warp-private: the warp lands its OWN block (the first passes of the inverse stay inside it)
-                    constexpr int BS = N / WP_NG;
-#pragma unroll
-                    for (int r = 0; r < BS / WP_TG; r++)
-                    {
-                        const int e = wwarp * BS + wlane + WP_TG * r;
-                        asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(smd + ntt_pad(e))), "l"(src + e)
-                                     : "memory");
-                    }
-                    asm volatile("cp.async.commit_group;" ::: "memory");
-                    asm volatile("cp.async.wait_group 0;" ::: "memory");
-                }
-                else
-                {
-#pragma unroll
-                    for (int it = 0; it < N / NT; it++)
-                        asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(sbase + (unsigned)(it * PNT * 8)), "l"(src + tid + it * NT)
-                                     : "memory");
-                    asm volatile("cp.async.commit_group;" ::: "memory");
-                    asm volatile("cp.async.wait_group 0;" ::: "memory");
-                }
+                __syncthreads();                                 // (by other threads)
             }
-            if (WP && !FWD && !STREAM && !job.tensor_mode && !(ABL & 2)) // (streaming: the block was requested by other threads)
-                wp_sync();
             else
-                __syncthreads();
-            if (job.timeline && tid == 0)
-            {
-                unsigned long long t;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-                job.timeline[(unsigned long long)blockIdx.x * 8 + 6] = t; // copy-in complete
+            { // the warp lands its OWN block (the first passes of the inverse stay inside it)
+                constexpr int BS = N / WP_NG;
+#pragma unroll
+                for (int r = 0; r < BS / WP_TG; r++)
+                {
+                    const int e = wwarp * BS + wlane + WP_TG * r;
+                    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(smd + ntt_pad(e))), "l"(src + e)
+                                 : "memory");
+                }
+                asm volatile("cp.async.commit_group;" ::: "memory");
+                asm volatile("cp.async.wait_group 0;" ::: "memory");
+                wp_sync();
             }
         }
-        constexpr bool RAW = EDGE_IN && !SG && !SMEM_IN; // (the tensor-fused copy-in writes doubles: handled by the run-time flag below)
+        constexpr bool RAW = EDGE_IN && !SG && !SMEM_IN;
         // renormalisation / input reduction are block-uniform run-time flags: branch ONCE to a compile-time variant
         // (as predicated code they cost 12 FP64 ops and ~10 IMADs per element whether needed or not)
-        // group handled by this thread in iteration `it`: block-strided by default, inside the warp's own block when warp-private
+        // group handled by this thread in iteration `it`: block-strided in the first forward and the last inverse pass, inside
+        // the warp's own block otherwise
         auto gidx = [&](int it) { return WPSTEP ? wwarp * (NGROUPS / WP_NG) + wlane + WP_TG * it : tid + it * NT; };
         auto groups = [&](auto RN, auto RD) {
-            if constexpr (STREAM && FWD && EDGE_OUT && !DG)
-            {
-                // streaming forward transform, last (sub-stride-1) pass: the 32 groups a warp handles in one iteration are one
-                // contiguous region of 32 R elements that no other warp touches in this pass, so the region is written out
-                // (coalesced, canonical) by the warp itself as soon as its groups are done — no block-wide barrier — and
-                // the NEXT polynomial's words for the same region are requested into the slots just read
-                constexpr int R = 1 << L;
-                static_assert(NGROUPS % NT == 0, "whole iterations");
-                const int lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-                for (int it = 0; it < ITERS; it++)
-                {
-                    const int g = tid + it * NT;
-                    ntt_fp_group<L, FWD, false, false, TW16, decltype(RN)::value, false, false, false, false, TWSRC, ABL>(
-                        smd, src, dst, g, LOGS, LOGN, M, P, true, false, true, PI_.p, PI_.ratio1, nullptr, nullptr, stw);
-                    __syncwarp();
-                    const int e0 = ((warp << 5) + it * NT) << L;
-#pragma unroll
-                    for (int r = 0; r < R; r++)
-                    {
-                        const int e = e0 + lane + 32 * r;
-                        const int pe = ntt_pad(e);
-                        dst[e] = fp_to_canonical<true>(smd[pe], P.p, P.pinv);
-                        if (nsrc)
-                            asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(smd + pe)), "l"(nsrc + e)
-                                         : "memory");
-                    }
-                }
-            }
-            else if constexpr (SG && NGROUPS % NT == 0 && ITERS > 1 && !GATHER)
+            if constexpr (SG && NGROUPS % NT == 0 && ITERS > 1 && !GATHER)
             {
                 // direct first pass, software-pipelined: the raw words of group it+1 are requested before group `it` is
                 // transformed, so one DRAM latency is exposed per polynomial instead of one per group
@@ -688,7 +571,7 @@ struct NttFpStaticPass
                     const int b0 = (i0 << (LOGS + L)) + o0;
 #pragma unroll
                     for (int j = 0; j < R; j++)
-                        cur[j] = (ABL & 2) ? (u64)(b0 + j) : (ABL & 8) ? __ldcs(src + b0 + (j << LOGS)) : src[b0 + (j << LOGS)];
+                        cur[j] = src[b0 + (j << LOGS)];
                 }
 #pragma unroll
                 for (int it = 0; it < ITERS; it++)
@@ -700,9 +583,9 @@ struct NttFpStaticPass
                         const int bn = (in_ << (LOGS + L)) + on;
 #pragma unroll
                         for (int j = 0; j < R; j++)
-                            nxt[j] = (ABL & 2) ? (u64)(bn + j) : (ABL & 8) ? __ldcs(src + bn + (j << LOGS)) : src[bn + (j << LOGS)];
+                            nxt[j] = src[bn + (j << LOGS)];
                     }
-                    ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, true, false, false, TWSRC, ABL>(
+                    ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, true, false, false, STW>(
                         smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, cur, nullptr, stw);
 #pragma unroll
                     for (int j = 0; j < R; j++)
@@ -724,85 +607,41 @@ struct NttFpStaticPass
 #pragma unroll
                     for (int j = 0; j < R; j++)
                         cur[j] = gather_ld(b0 + (j << LOGS));
-                    ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, true, false, false, TWSRC, ABL>(
+                    ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, true, false, false, STW>(
                         smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, cur, nullptr, stw);
+                }
+            }
+            else if constexpr (L <= 3 && NGROUPS % NT == 0 && ITERS > 1 && !STW)
+            {
+                // the twiddles of group it+1 are requested before group `it` is transformed: their L1/L2 latency
+                // (the kernel's largest stall reason when profiled) overlaps the butterflies
+                constexpr int R = 1 << L;
+                const double *__restrict__ twt = FWD ? P.fwd : P.inv;
+                double twc[R - 1], twn[R - 1];
+                fp_load_group_tw<L, FWD, false>(twc, twt, gidx(0), gidx(0) >> LOGS, LOGS, LOGN, M, 0, P, !FWD && EDGE_OUT);
+#pragma unroll
+                for (int it = 0; it < ITERS; it++)
+                {
+                    const int g = gidx(it);
+                    if (it + 1 < ITERS)
+                        fp_load_group_tw<L, FWD, false>(twn, twt, gidx(it + 1), gidx(it + 1) >> LOGS, LOGS, LOGN, M, 0, P, !FWD && EDGE_OUT);
+                    ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, false, RAW, true, false, STREAM && DG>(
+                        smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, nullptr, twc, nullptr, nsrc);
+#pragma unroll
+                    for (int j = 0; j < R - 1; j++)
+                        twc[j] = twn[j];
                 }
             }
             else
             {
-                auto run = [&](auto RAWF) {
-                    if constexpr ((VAR & 1024) != 0 && L <= 3 && NGROUPS % NT == 0 && ITERS > 1 && !decltype(RAWF)::value)
-                    {
-                        // VAR & 1024: the DATA of group it+1 is read from shared memory before group `it` is transformed (instead of
-                        // prefetching twiddles): hides the shared-memory latency / queueing behind the butterflies
-                        constexpr int R = 1 << L;
-                        u64 xc[R], xn[R];
-                        auto fetch = [&](u64(&dstv)[R], int g) {
-                            const int i_ = g >> LOGS, o_ = g & ((1 << LOGS) - 1);
-                            const int b_ = (i_ << (LOGS + L)) + o_;
-                            const int pb_ = ntt_pad(b_);
 #pragma unroll
-                            for (int j = 0; j < R; j++)
-                                dstv[j] = (u64)__double_as_longlong(smd[fp_elem_index(pb_, b_, j, LOGS)]);
-                        };
-                        fetch(xc, gidx(0));
-#pragma unroll
-                        for (int it = 0; it < ITERS; it++)
-                        {
-                            const int g = gidx(it);
-                            if (it + 1 < ITERS)
-                                fetch(xn, gidx(it + 1));
-                            ntt_fp_group<L, FWD, false, DG, TW16, decltype(RN)::value, false, true, false, false, TWSRC, ABL, STREAM && !FWD && DG>(
-                                smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, xc, nullptr, stw, nsrc);
-#pragma unroll
-                            for (int j = 0; j < R; j++)
-                                xc[j] = xn[j];
-                        }
-                    }
-                    else if constexpr (L <= 3 && NGROUPS % NT == 0 && ITERS > 1 && B200_NTT_TW_PREFETCH && TWSRC == 0)
-                    {
-                        // the twiddles of group it+1 are requested before group `it` is transformed: their L1/L2 latency
-                        // (the kernel's largest stall reason when profiled) overlaps the butterflies
-                        constexpr int R = 1 << L;
-                        const double *__restrict__ twt = FWD ? P.fwd : P.inv;
-                        double twc[R - 1], twn[R - 1];
-                        fp_load_group_tw<L, FWD, false>(twc, twt, gidx(0), gidx(0) >> LOGS, LOGS, LOGN, M, 0, P, !FWD && EDGE_OUT);
-#pragma unroll
-                        for (int it = 0; it < ITERS; it++)
-                        {
-                            const int g = gidx(it);
-                            if (it + 1 < ITERS)
-                                fp_load_group_tw<L, FWD, false>(twn, twt, gidx(it + 1), gidx(it + 1) >> LOGS, LOGS, LOGN, M, 0, P, !FWD && EDGE_OUT);
-                            ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, false, decltype(RAWF)::value, true, 0, ABL,
-                                         STREAM && !FWD && DG>(
-                                smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, nullptr, twc, nullptr, nsrc);
-#pragma unroll
-                            for (int j = 0; j < R - 1; j++)
-                                twc[j] = twn[j];
-                        }
-                    }
-                    else
-                    {
-#pragma unroll
-                        for (int it = 0; it < ITERS; it++)
-                        {
-                            const int g = gidx(it);
-                            if (NGROUPS % NT == 0 || g < NGROUPS)
-                                ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, false, decltype(RAWF)::value, false, TWSRC, ABL,
-                                             STREAM && !FWD && DG>(
-                                    smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, nullptr, nullptr, stw, nsrc);
-                        }
-                    }
-                };
-                if constexpr (RAW)
+                for (int it = 0; it < ITERS; it++)
                 {
-                    if (!FWD && job.tensor_mode)
-                        run(std::false_type{});
-                    else
-                        run(std::true_type{});
+                    const int g = gidx(it);
+                    if (NGROUPS % NT == 0 || g < NGROUPS)
+                        ntt_fp_group<L, FWD, SG, DG, TW16, decltype(RN)::value, decltype(RD)::value, false, RAW, false, STW, STREAM && DG>(
+                            smd, src, dst, g, LOGS, LOGN, M, P, true, !FWD && EDGE_OUT, true, PI_.p, PI_.ratio1, nullptr, nullptr, stw, nsrc);
                 }
-                else
-                    run(std::false_type{});
             }
         };
         if (rn)
@@ -823,46 +662,19 @@ struct NttFpStaticPass
             wp_sync(); // the next pass (or the write-out) of this group touches only the group's own block(s)
         else if (!(STREAM && EDGE_OUT)) // (the streaming kernel's next polynomial starts with wait_all + barrier)
             __syncthreads();
-        if (job.timeline && tid == 0)
-        {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-            job.timeline[(unsigned long long)blockIdx.x * 8 + 2 + STEP] = t;
-        }
-        if (EDGE_OUT && !DG && !(STREAM && FWD) && !KEEP_OUT)
-        { // coalesced copy-out: lazy double -> canonical u64
-            if constexpr ((VAR & 256) != 0)
-            { // two adjacent words per thread: one 128-bit store (the pair never straddles a pad: even index, runs of 16)
+        if constexpr (EDGE_OUT && !DG && !KEEP_OUT)
+        { // coalesced copy-out (lazy double -> canonical u64): the warp writes its own block out as soon as its last pass is
+          // done (no block-wide barrier before this)
+            constexpr int BS = N / WP_NG;
 #pragma unroll
-                for (int it = 0; it < N / (2 * NT); it++)
-                {
-                    const int e = 2 * (tid + it * NT);
-                    const int pe = ntt_pad(e);
-                    const u64 v0 = fp_to_canonical<true>(smd[pe], P.p, P.pinv), v1 = fp_to_canonical<true>(smd[pe + 1], P.p, P.pinv);
-                    __stcs(reinterpret_cast<ulonglong2 *>(dst + e), make_ulonglong2(v0, v1));
-                }
-            }
-            else if constexpr (WP)
-            { // the warp writes its own block out as soon as its last pass is done (no block-wide barrier before this)
-                constexpr int BS = N / WP_NG;
-#pragma unroll
-                for (int r = 0; r < BS / WP_TG; r++)
-                {
-                    const int e = wwarp * BS + wlane + WP_TG * r;
-                    dst[e] = fp_to_canonical<true>(smd[ntt_pad(e)], P.p, P.pinv);
-                }
-            }
-            else
-#pragma unroll
-            for (int it = 0; it < N / NT; it++)
+            for (int r = 0; r < BS / WP_TG; r++)
             {
-                const u64 v = fp_to_canonical<true>(smd[ptid + it * PNT], P.p, P.pinv);
-                if (!(ABL & 4) || v == 0xFFFFFFFFFFFFFFFFULL)
-                    dst[tid + it * NT] = v;
+                const int e = wwarp * BS + wlane + WP_TG * r;
+                dst[e] = fp_to_canonical<true>(smd[ntt_pad(e)], P.p, P.pinv);
             }
         }
         if (STEP + 1 < NP)
-            NttFpStaticPass<LOGN, NT, FWD, (STEP + 1 < NP ? STEP + 1 : STEP), VAR>::run(job, P, PI_, src, dst, smd, tid, item, slot, nsrc, gal, gal_q);
+            NttFpStaticPass<LOGN, NT, FWD, (STEP + 1 < NP ? STEP + 1 : STEP), OPT>::run(job, P, PI_, src, dst, smd, tid, nsrc, gal, gal_q);
 #endif
     }
 };

@@ -1,21 +1,29 @@
 // ntt_fp_kernels.cu — the statically scheduled FP64-pipe NTT / INTT kernels (ntt_fp_body.cuh) as their own translation
-// unit: every (size, direction, CTA width, variant) instantiation is compiled here once; b200_bfv.cu launches them through
+// unit: every (size, direction, CTA width) kernel is compiled here once; b200_bfv.cu launches them through
 // the function pointers returned by b200_ntt_fp_kernel().
 #include "ntt_fp_kernels.h"
 #include "ntt_fp_body.cuh"
 #include <cuda_runtime.h>
 
-// FP64-only statically scheduled kernel (all slots of the job use FP-capable primes)
-template <int LOGN, bool FWD, int NT, int VAR>
+// The options each transform ships with, per (log2 n, direction): every pass after the first forward (before the last inverse)
+// one is warp-private; the n = 8192 inverse and the n = 16384 forward read the first twiddles from shared memory, and the
+// n = 16384 inverse is the persistent kernel whose input streams in during the previous polynomial's last pass.
+template <int LOGN, bool FWD>
+using KernelOpt = NttFpOpt<(LOGN == 13 && !FWD) || (LOGN == 14 && FWD), LOGN == 14 && !FWD>;
+
+// FP64-only statically scheduled kernel (all slots of the job use FP-capable primes).  Blocks run slot-major (all items of
+// slot 0, then slot 1, ...): CTAs that run at the same time work on the same prime, so the early-pass twiddles stay in L1.
+template <int LOGN, bool FWD, int NT>
 __global__ void __launch_bounds__(NT, (LOGN <= 13 ? (NT <= 256 ? 3 : 2) : 1)) ntt_fp_kernel(const NttJob job)
 {
+    using OPT = KernelOpt<LOGN, FWD>;
     extern __shared__ u64 ntt_sm[];
-    if constexpr ((VAR & 16) != 0)
+    if constexpr (OPT::STREAM)
     {
-        // Streaming variant: a persistent CTA walks blockIdx.x, blockIdx.x + gridDim.x, ... ; while one polynomial's LAST pass
-        // runs, the next polynomial's words are already requested (cp.async) into the shared-memory slots that pass has
-        // finished with, so no CTA ever sits idle waiting for its input (tools/ntt_ablate.py: with global traffic removed the
-        // same kernel needs 0.49 ms instead of 0.70 ms for 16384 transforms — that wait is what this variant hides).
+        // Persistent CTAs walk blockIdx.x, blockIdx.x + gridDim.x, ... ; while one polynomial's LAST pass runs, the next
+        // polynomial's words are already requested (cp.async) into the shared-memory slots that pass has finished with, so no
+        // CTA ever sits idle waiting for its input (with global traffic removed the same kernel needed 0.49 ms instead of
+        // 0.70 ms for 16384 transforms — that wait is what this kernel hides).
         constexpr int N = 1 << LOGN;
         const long long total = job.items * (long long)job.slots;
         long long b = (long long)blockIdx.x;
@@ -23,15 +31,8 @@ __global__ void __launch_bounds__(NT, (LOGN <= 13 ? (NT <= 256 ? 3 : 2) : 1)) nt
             return;
         const int tid = (int)threadIdx.x;
         double *smd = reinterpret_cast<double *>(ntt_sm);
-        if (job.stagger > 0 && job.sm_count > 0)
-        { // persistent CTAs would otherwise march in lockstep: all loading, then all computing
-            const long long wait = (long long)(blockIdx.x / (unsigned)job.sm_count) * job.stagger;
-            const long long t0 = clock64();
-            while (clock64() - t0 < wait)
-                ;
-        }
-        int slot = job.slot_major ? (int)(b / job.items) : (int)(b % job.slots);
-        long long item = job.slot_major ? b - (long long)slot * job.items : b / job.slots;
+        int slot = (int)(b / job.items);
+        long long item = b - (long long)slot * job.items;
         const u64 *src = ntt_src_ptr(job, item, slot);
         {
             const int ptid = ntt_pad(tid);
@@ -53,11 +54,11 @@ __global__ void __launch_bounds__(NT, (LOGN <= 13 ? (NT <= 256 ? 3 : 2) : 1)) nt
             long long nitem = 0;
             if (nb < total)
             {
-                nslot = job.slot_major ? (int)(nb / job.items) : (int)(nb % job.slots);
-                nitem = job.slot_major ? nb - (long long)nslot * job.items : nb / job.slots;
+                nslot = (int)(nb / job.items);
+                nitem = nb - (long long)nslot * job.items;
                 nsrc = ntt_src_ptr(job, nitem, nslot);
             }
-            NttFpStaticPass<LOGN, NT, FWD, 0, VAR>::run(job, PF, PI_, src, dst, smd, tid, item, slot, nsrc);
+            NttFpStaticPass<LOGN, NT, FWD, 0, OPT>::run(job, PF, PI_, src, dst, smd, tid, nsrc);
             if (!nsrc)
                 break;
             b = nb;
@@ -68,67 +69,45 @@ __global__ void __launch_bounds__(NT, (LOGN <= 13 ? (NT <= 256 ? 3 : 2) : 1)) nt
         return;
     }
     const long long block = (long long)blockIdx.x;
-    // slot-major order: CTAs that run at the same time work on the same prime, so the early-pass twiddles stay in L1
-    const int slot = job.slot_major ? (int)(block / job.items) : (int)(block % job.slots);
-    const long long item = job.slot_major ? block - (long long)slot * job.items : block / job.slots;
+    const int slot = (int)(block / job.items);
+    const long long item = block - (long long)slot * job.items;
     const int pidx = job.slot_prime[slot];
     const NttPrimeFp PF = job.fprimes[pidx];
     const NttPrime PI_ = job.primes[pidx];
     const u64 *src = ntt_src_ptr(job, item, slot);
     u64 *dst = job.dst + item * job.dst_item_stride + job.slot_dst[slot];
-    if (job.timeline && threadIdx.x == 0)
-    {
-        unsigned long long t;
-        unsigned smid;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        job.timeline[block * 8] = smid;
-        job.timeline[block * 8 + 1] = t;
-    }
-    if (job.prefetch_dist > 0 && !job.tensor_mode)
-    {
-        // pull the polynomial that the CTA one wave later will transform into L2 (its pass-1 loads then hit L2)
-        const long long nb = block + job.prefetch_dist;
-        if (nb < (long long)gridDim.x)
-        {
-            const int nslot = job.slot_major ? (int)(nb / job.items) : (int)(nb % job.slots);
-            const long long nitem = job.slot_major ? nb - (long long)nslot * job.items : nb / job.slots;
-            const char *np_ = reinterpret_cast<const char *>(ntt_src_ptr(job, nitem, nslot));
-            constexpr int LINES = (8 << LOGN) / 128;
-#pragma unroll
-            for (int l = (int)threadIdx.x; l < LINES; l += NT)
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(np_ + (size_t)l * 128));
-        }
-    }
-    NttFpStaticPass<LOGN, NT, FWD, 0, VAR>::run(job, PF, PI_, src, dst, reinterpret_cast<double *>(ntt_sm), (int)threadIdx.x, item, slot);
-    if (job.timeline && threadIdx.x == 0)
-    {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        job.timeline[block * 8 + 7] = t;
-    }
+    NttFpStaticPass<LOGN, NT, FWD, 0, OPT>::run(job, PF, PI_, src, dst, reinterpret_cast<double *>(ntt_sm), (int)threadIdx.x);
 }
 
+// (log2 n, threads per CTA) of every kernel, each in both directions: the n = 8192 transform has a 256-thread (throughput)
+// and a 512-thread (latency) width
+#define B200_FP_KERNELS(X) X(12, 256) X(13, 256) X(13, 512) X(14, 1024)
 
-#define B200_FP_KERNELS(X)                                                                                             \
-    X(12, 256, 0) X(12, 256, 1)                                                                                        \
-    X(13, 256, 0) X(13, 256, 1) X(13, 512, 0) X(13, 512, 1)                                                            \
-    X(14, 1024, 0) X(14, 1024, 1)                                                                                      \
-    /* developer ablations (tools/ntt_ablate.py), n = 8192 throughput configuration only */                            \
-    X(13, 256, 2) X(13, 256, 4) X(13, 256, 6) X(13, 256, 8) X(13, 256, 14) X(13, 256, 32) X(13, 256, 64) X(13, 256, 128) X(13, 256, 256) X(13, 256, 384) X(13, 256, 512) X(13, 256, 896) X(13, 256, 1024) X(13, 256, 1025)                                                                           \
-    /* warp-private sub-transforms (+ streaming inverse) */                                                             \
-    X(12, 256, 2048) X(12, 256, 2049) X(13, 512, 2048) X(13, 512, 2049) X(13, 256, 2048) X(13, 256, 2064) X(13, 256, 2049) X(14, 1024, 2048) X(14, 1024, 2049) X(14, 1024, 2064)                                             \
-    /* streaming (persistent) variant */                                                                               \
-    X(12, 256, 16) X(13, 256, 16) X(14, 1024, 16)
-
-b200_ntt_fp_fn b200_ntt_fp_kernel(int logn, bool fwd, int nt, int var)
+b200_ntt_fp_fn b200_ntt_fp_kernel(int logn, bool fwd, int nt)
 {
-#define X(LOGN, NT, VAR)                                                                                               \
-    if (logn == LOGN && nt == NT && var == VAR)                                                                        \
-        return fwd ? ntt_fp_kernel<LOGN, true, NT, VAR> : ntt_fp_kernel<LOGN, false, NT, VAR>;
+#define X(LOGN, NT)                                                                                                    \
+    if (logn == LOGN && nt == NT)                                                                                      \
+        return fwd ? ntt_fp_kernel<LOGN, true, NT> : ntt_fp_kernel<LOGN, false, NT>;
     B200_FP_KERNELS(X)
 #undef X
     return nullptr;
+}
+
+template <int LOGN, bool FWD>
+static B200NttFpLayout fp_layout()
+{
+    using OPT = KernelOpt<LOGN, FWD>;
+    const size_t words = (size_t)ntt_smem_words(1 << LOGN) + (OPT::SMEM_TW ? B200_NTT_TWS_ENTRIES : 0);
+    return B200NttFpLayout{ words * sizeof(double), OPT::STREAM };
+}
+
+B200NttFpLayout b200_ntt_fp_layout(int logn, bool fwd)
+{
+    if (logn == 12)
+        return fwd ? fp_layout<12, true>() : fp_layout<12, false>();
+    if (logn == 13)
+        return fwd ? fp_layout<13, true>() : fp_layout<13, false>();
+    return fwd ? fp_layout<14, true>() : fp_layout<14, false>();
 }
 
 int b200_ntt_fp_ctas_per_sm(b200_ntt_fp_fn fn, int nt, size_t smem)
@@ -142,11 +121,11 @@ int b200_ntt_fp_ctas_per_sm(b200_ntt_fp_fn fn, int nt, size_t smem)
 int b200_ntt_fp_setup(int smem_optin)
 {
     cudaError_t e;
-#define X(LOGN, NT, VAR)                                                                                               \
-    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, true, NT, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin)) != cudaSuccess) return (int)e; \
-    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, false, NT, VAR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin)) != cudaSuccess) return (int)e; \
-    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, true, NT, VAR>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)) != cudaSuccess) return (int)e; \
-    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, false, NT, VAR>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)) != cudaSuccess) return (int)e;
+#define X(LOGN, NT)                                                                                                    \
+    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, true, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin)) != cudaSuccess) return (int)e; \
+    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, false, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin)) != cudaSuccess) return (int)e; \
+    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, true, NT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)) != cudaSuccess) return (int)e; \
+    if ((e = cudaFuncSetAttribute(ntt_fp_kernel<LOGN, false, NT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100)) != cudaSuccess) return (int)e;
     B200_FP_KERNELS(X)
 #undef X
     return 0;

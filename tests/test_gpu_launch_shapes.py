@@ -1,14 +1,13 @@
-"""Launch shapes and kernel variants the fixed-size parity tests do not pick on purpose (pytest -m gpu).
+"""Launch shapes the fixed-size parity tests do not pick on purpose (pytest -m gpu).
 
 Every batch size here is derived from the device's SM count and the host-side launch formulas it targets, so the same
 boundaries are hit on any H100 configuration:
   * n = 8192 static NTT: 512 threads per CTA while items * k <= 2 * sm_count, 256 above (b200_bfv.cu launch_ntt);
-  * n = 16384 inverse NTT: the persistent variant runs min(blocks, per_sm * sm_count) CTAs, each prefetching the next
+  * n = 16384 inverse NTT: the persistent kernel runs min(blocks, per_sm * sm_count) CTAs, each prefetching the next
     polynomial it walks to, which may belong to another prime (ntt_fp_kernels.cu);
   * the key-switch MAC (ksmac_tma.cu launch): the batch is cut into chunks of `ipc` items whose last one is partial unless
     ipc divides the batch;
-  * every correct FP64 NTT variant of every instantiated (size, CTA width), forced through b200_debug_ntt_variant;
-  * settings read once per process (fused tensor inverse, the non-TMA key-switch MAC) in a subprocess each.
+  * a setting read once per process (the non-TMA key-switch MAC) in a subprocess.
 Every output word is compared with the unmodified reference."""
 import os
 import re
@@ -47,10 +46,10 @@ def _threads():
     return max(1, min(64, len(os.sched_getaffinity(0))))
 
 
-def persistent_ctas_per_sm(P, nt, var, forward=False):
+def persistent_ctas_per_sm(P, nt, forward=False):
     """resident CTAs per SM of an FP64 NTT kernel: the occupancy query the launcher makes to cap the persistent
-    variant's grid (b200_debug_ntt_ctas_per_sm)"""
-    per_sm = P.be.lib.lib.b200_debug_ntt_ctas_per_sm(P.n.bit_length() - 1, int(forward), nt, var)
+    kernel's grid (b200_debug_ntt_ctas_per_sm)"""
+    per_sm = P.be.lib.lib.b200_debug_ntt_ctas_per_sm(P.n.bit_length() - 1, int(forward), nt)
     assert per_sm >= 1, per_sm
     return per_sm
 
@@ -107,7 +106,7 @@ def test_n8192_ntt_thread_count_boundary(pairs, side):
 # n = 16384: persistent inverse NTT at grids below, at and well above its CTA cap, and multiply_relin around it
 # ---------------------------------------------------------------------------------------------------------------------
 def _n16384_grid(P):
-    return persistent_ctas_per_sm(P, 1024, 2064) * P.ctx.sm_count
+    return persistent_ctas_per_sm(P, 1024) * P.ctx.sm_count
 
 
 @pytest.mark.parametrize("side", ["below", "at", "above"])
@@ -182,50 +181,18 @@ def test_ksmac_partial_last_chunk_runs_the_tma_kernel(ref):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# every correct FP64 NTT variant, forced
+# the FP64 NTT kernel table
 # ---------------------------------------------------------------------------------------------------------------------
-CORRECT_VARIANTS = (0, 1, 16, 2048, 2049, 2064)    # the others at (13, 256) are timing ablations with meaningless output
-SIZE_SET = {12: "n4096", 13: "n8192", 14: "n16384"}
-
-
-def instantiated_variants():
-    """(logn, threads per CTA, variant) of every correct instantiation in ntt_fp_kernels.cu (B200_FP_KERNELS)"""
+def test_kernel_table_has_the_four_shapes():
+    """ntt_fp_kernels.cu instantiates exactly one kernel per (size, CTA width) and direction: the widths launch_ntt picks"""
     src = open(os.path.join(ROOT, "sunscreen_b200", "csrc", "ntt_fp_kernels.cu")).read()
-    block = src[src.index("#define B200_FP_KERNELS"):src.index("b200_ntt_fp_fn b200_ntt_fp_kernel")]
-    found = sorted({tuple(map(int, m)) for m in re.findall(r"X\((\d+), (\d+), (\d+)\)", block)})
-    return [f for f in found if f[2] in CORRECT_VARIANTS]
-
-
-VARIANTS = instantiated_variants()
-
-
-def test_variant_table_covers_every_size():
-    assert {(l, nt) for l, nt, _ in VARIANTS} == {(12, 256), (13, 256), (13, 512), (14, 1024)}
-    assert {v for _, _, v in VARIANTS} == set(CORRECT_VARIANTS)
-
-
-@pytest.mark.parametrize("logn,nt,var", VARIANTS)
-def test_forced_ntt_variant(be, pairs, logn, nt, var):
-    P = pairs(SIZE_SET[logn])
-    sm = P.ctx.sm_count
-    if logn == 13 and nt == 512:
-        items = max(6, (2 * sm) // P.k // 2)             # stays at or below 2 * sm_count blocks
-        assert items * P.k <= 2 * sm
-    elif var & 16:
-        items = -(-3 * persistent_ctas_per_sm(P, nt, var) * sm // P.k) + 1   # every persistent CTA walks >= 3 polys
-    else:
-        items = 2 * sm // P.k + 3                         # above the 512-thread limit at n = 8192
-    L = be.lib.lib
-    old = L.b200_debug_ntt_variant(var)
-    try:
-        pc.check_ntt(P, items=items, seed=var + logn)
-        pc.check_relin(P)
-    finally:
-        L.b200_debug_ntt_variant(old)
+    line = next(ln for ln in src.splitlines() if ln.startswith("#define B200_FP_KERNELS"))
+    shapes = [tuple(map(int, m)) for m in re.findall(r"X\((\d+), (\d+)\)", line)]
+    assert shapes == [(12, 256), (13, 256), (13, 512), (14, 1024)]
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# settings read once per process
+# a setting read once per process
 # ---------------------------------------------------------------------------------------------------------------------
 _SUBPROCESS_CHECKS = """
 import sys
@@ -248,7 +215,7 @@ for name in ("n4096", "n8192", "n16384"):
 """
 
 
-@pytest.mark.parametrize("setting", ["B200_TENSOR_FUSION=1", "B200_KSMAC_TMA=0"])
+@pytest.mark.parametrize("setting", ["B200_KSMAC_TMA=0"])
 def test_process_wide_setting(ref, setting):
     name, value = setting.split("=")
     env = dict(os.environ, **{name: value})

@@ -230,7 +230,7 @@ for j in (T.data_levels(P) if {every} else [0]):
 def traced_levels(name, every=True):
     """[(op, j, k, fused, launches)] of relinearize and multiply_relin at every data level (or the top one) of `name`"""
     env = dict(os.environ, B200_TRACE="1")
-    for var in ("B200_KS_CLUSTER", "B200_MUL_CLUSTER", "B200_TENSOR_FUSION", "B200_KSMAC_TMA", "B200_MR_SPLIT",
+    for var in ("B200_KS_CLUSTER", "B200_MUL_CLUSTER", "B200_KSMAC_TMA", "B200_MR_SPLIT",
                 "B200_FORCE_AUX61", "B200_NO_STATIC_NTT"):
         env.pop(var, None)
     cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + \

@@ -159,7 +159,7 @@ P.be.lib.lib.b200_trace_dump()
 
 def traced_launches(name, side, **env_extra):
     env = dict(os.environ, B200_TRACE="1", **env_extra)
-    for var in ("B200_TENSOR_FUSION", "B200_MUL_CLUSTER"):
+    for var in ("B200_MUL_CLUSTER",):
         if var not in env_extra:
             env.pop(var, None)
     cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + \

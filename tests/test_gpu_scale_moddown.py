@@ -163,7 +163,7 @@ P.be.lib.lib.b200_trace_dump()
 
 def traced_multiply_relin(name, j, batch):
     env = dict(os.environ, B200_TRACE="1")
-    for var in ("B200_MR_SPLIT", "B200_KS_CLUSTER", "B200_MUL_CLUSTER", "B200_TENSOR_FUSION"):
+    for var in ("B200_MR_SPLIT", "B200_KS_CLUSTER", "B200_MUL_CLUSTER"):
         env.pop(var, None)
     cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + \
         ["-c", _TRACE.format(root=ROOT, tests=HERE, name=name, j=j, batch=batch)]

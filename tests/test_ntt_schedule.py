@@ -5,13 +5,13 @@ instantiated shape without a GPU:
   * after the first forward pass (before the last inverse pass) the groups a warp group handles touch ONLY the elements of that
     group's own block(s), in every remaining pass — which is why a __syncwarp / named barrier of that group is enough between them;
   * the write-out / copy-in of a group covers exactly its block(s).
-The kernels themselves are compared bit for bit with the reference by tests/test_gpu_launch_shapes.py, which forces each
-correct variant (0, 1, 16, 2048, 2049, 2064) of every instantiated shape through b200_debug_ntt_variant; the timing
-ablations are left out."""
+The kernels themselves are compared bit for bit with the reference by the GPU parity tests, whose batch sizes reach every
+shape through the launcher's automatic choice (tests/test_gpu_launch_shapes.py: both sides of the n = 8192 width switch and
+of the n = 16384 persistent grid)."""
 import pytest
 
 SCHED = {12: (4, 4, 4), 13: (3, 3, 3, 4), 14: (3, 3, 4, 4)}   # NttSched<LOGN>: stages per forward pass
-SHAPES = [(12, 256), (13, 256), (13, 512), (14, 1024)]          # (LOGN, threads per CTA) instantiated with the WP variants
+SHAPES = [(12, 256), (13, 256), (13, 512), (14, 1024)]          # (LOGN, threads per CTA) of the kernels (ntt_fp_kernels.cu)
 
 
 def wp_geometry(logn, nt):
