@@ -56,6 +56,28 @@ static inline bool trace_on()
         else                                                                                                           \
             kernel<<<grid, block, smem, stream>>>(__VA_ARGS__);                                                        \
     } while (0)
+// The trace of a launch that B200_LAUNCH cannot wrap: `launch` is a host call that launches on `stream` and returns 0, or
+// non-zero when it failed or launched nothing; only a launch that returned 0 is recorded, under `name`.
+template <class F>
+static int traced_launch(const char *name, cudaStream_t stream, F &&launch)
+{
+    if (!trace_on())
+        return launch();
+    B200TraceRec r{ name, nullptr, nullptr };
+    cudaEventCreate(&r.e0);
+    cudaEventCreate(&r.e1);
+    cudaEventRecord(r.e0, stream);
+    const int rc = launch();
+    if (rc)
+    {
+        cudaEventDestroy(r.e0);
+        cudaEventDestroy(r.e1);
+        return rc;
+    }
+    cudaEventRecord(r.e1, stream);
+    g_trace.push_back(r);
+    return 0;
+}
 #endif
 #include <condition_variable>
 #include <functional>
@@ -412,31 +434,13 @@ __global__ void ksmac_kernel_v2(const NttPrimeFp *fprimes, int special_idx, int 
     stg2(o1, fp_to_canonical(acc[0][1], p, pinv), fp_to_canonical(acc[1][1], p, pinv));
 }
 
-template <int K>
-__global__ void ksmoddown_kernel(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *ks2,
-                                 const u64 *base0, long long base0_stride, const u64 *base1, long long base1_stride,
-                                 u64 *dst, long long dst_item_stride, long long n, long long total)
-{
-    const long long idx = GLOBAL_IDX();
-    if (idx >= total)
-        return;
-    const long long c = idx % n;
-    const long long t = idx / n;
-    const int comp = (int)(t & 1);
-    const long long item = t >> 1;
-    const PrimeDev SP = ld_prime(&primes[special_idx]);
-    const u64 *acc = ks2 + ((item * 2 + comp) * (K + 1)) * n;
-    const u64 *base = comp == 0 ? (base0 ? base0 + item * base0_stride : nullptr)
-                                : (base1 ? base1 + item * base1_stride : nullptr);
-    u64 *d = dst + item * dst_item_stride + (long long)comp * K * n;
-    ksmoddown_coeff<K>(primes, SP, inv_qsp, acc, n, base, d, c);
-}
-
-// the key-switch mod-down of two adjacent coefficients: acc = the k + 1 ks2 rows of one component at coefficient c;
-// d row i = moddown(acc)_i + base[.][i] (mod q_i), base canonical
-template <int K>
-B200_DEV void ksmoddown2(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *acc, long long n,
-                         const u64 (&base)[2][K], u64 *d)
+// the key-switch mod-down of two adjacent coefficients, kept in registers: acc = the k + 1 ks2 rows of one component at
+// coefficient c; x[u][i] <- moddown(acc)_i + x[u][i] (mod q_i), x canonical.  STORE: each row x[.][i] is also stored to
+// d + i n as soon as it is formed (storing after the loop instead holds all 2K words live and costs registers).
+//   s = [acc_sp + floor(q_sp/2)]_{q_sp};  moddown(acc)_i = (acc_i - [s]_{q_i} + [floor(q_sp/2)]_{q_i}) * q_sp^-1   (mod q_i)
+template <int K, bool STORE = false>
+B200_DEV void ksmoddown2_regs(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *acc, long long n,
+                              u64 (&x)[2][K], u64 *d = nullptr)
 {
     const PrimeDev SP = ld_prime(&primes[special_idx]);
     const u64 half = SP.p >> 1;
@@ -455,11 +459,23 @@ B200_DEV void ksmoddown2(const PrimeDev *primes, int special_idx, const u64 *inv
         u64 v1 = a.y + (Q.p - barrett64(s1, Q.p, Q.r1)) + h;
         v0 = shoup_mul(v0, w, wq, Q.p);
         v1 = shoup_mul(v1, w, wq, Q.p);
-        stg2(d + (long long)i * n, add_mod(v0, base[0][i], Q.p), add_mod(v1, base[1][i], Q.p));
+        u64 *const row = STORE ? d + (long long)i * n : nullptr;
+        x[0][i] = add_mod(v0, x[0][i], Q.p);
+        x[1][i] = add_mod(v1, x[1][i], Q.p);
+        if (STORE)
+            stg2(row, x[0][i], x[1][i]);
     }
 }
 
-// ksmoddown_kernel with two adjacent coefficients per thread: 128-bit loads / stores (the kernel is a pure stream of
+// ksmoddown2_regs with the result stored: d row i = moddown(acc)_i + base[.][i] (mod q_i)
+template <int K>
+B200_DEV void ksmoddown2(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *acc, long long n,
+                         u64 (&base)[2][K], u64 *d)
+{
+    ksmoddown2_regs<K, true>(primes, special_idx, inv_qsp, acc, n, base, d);
+}
+
+// the key-switch mod-down with two adjacent coefficients per thread: 128-bit loads / stores (the kernel is a pure stream of
 // 2(k+1) + k rows in, 2k rows out per item)
 template <int K>
 __global__ void ksmoddown_kernel_v2(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *ks2,
@@ -545,34 +561,6 @@ __global__ void ksmoddown_galois_add_kernel(const PrimeDev *primes, int special_
         b[1][i] = v.y;
     }
     ksmoddown2<K>(primes, special_idx, inv_qsp, ks2 + ((item * 2 + comp) * (K + 1)) * n + c, n, b, dst2 + off + c);
-}
-
-// ksmoddown2 with the result kept in registers: x[u][i] <- moddown(acc)_i + x[u][i] (mod q_i), x canonical.  The arithmetic is
-// ksmoddown2's word for word; only the store is replaced.
-template <int K>
-B200_DEV void ksmoddown2_regs(const PrimeDev *primes, int special_idx, const u64 *inv_qsp, const u64 *acc, long long n,
-                              u64 (&x)[2][K])
-{
-    const PrimeDev SP = ld_prime(&primes[special_idx]);
-    const u64 half = SP.p >> 1;
-    const b200_u64x2 sp = ldg2(acc + (long long)K * n);
-    u64 s0 = sp.x + half, s1 = sp.y + half;
-    s0 = s0 >= SP.p ? s0 - SP.p : s0;
-    s1 = s1 >= SP.p ? s1 - SP.p : s1;
-#pragma unroll
-    for (int i = 0; i < K; i++)
-    {
-        const PrimeDev Q = ld_prime(&primes[i]);
-        const u64 h = barrett64(half, Q.p, Q.r1);
-        const u64 w = B200_LDG(&inv_qsp[2 * i]), wq = B200_LDG(&inv_qsp[2 * i + 1]);
-        const b200_u64x2 a = ldg2(acc + (long long)i * n);
-        u64 v0 = a.x + (Q.p - barrett64(s0, Q.p, Q.r1)) + h;
-        u64 v1 = a.y + (Q.p - barrett64(s1, Q.p, Q.r1)) + h;
-        v0 = shoup_mul(v0, w, wq, Q.p);
-        v1 = shoup_mul(v1, w, wq, Q.p);
-        x[0][i] = add_mod(v0, x[0][i], Q.p);
-        x[1][i] = add_mod(v1, x[1][i], Q.p);
-    }
 }
 
 // b200_multiply_relin_sum's mod-down: out[u] = addend[u] + sum_{j < m} (base_j + moddown(ks2_j)) over the m items of output u,
@@ -2019,21 +2007,9 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
             job.primes = ctx->d_ntt_primes;
             job.fprimes = ctx->d_fp_primes;
             job.items = batch;
-            cudaEvent_t t0 = nullptr, t1 = nullptr;
-            if (trace_on())
-            {
-                cudaEventCreate(&t0);
-                cudaEventCreate(&t1);
-                cudaEventRecord(t0, s);
-            }
-            const int crc = b200_mul_cluster(ctx->logn, job, a, b, ext, D, k, s);
+            const int crc = traced_launch("mul_cluster_kernel", s, [&] { return b200_mul_cluster(ctx->logn, job, a, b, ext, D, k, s); });
             if (crc)
                 return fail(B200_E_CUDA, std::string("mul_cluster_kernel: ") + cudaGetErrorString((cudaError_t)crc));
-            if (t0)
-            {
-                cudaEventRecord(t1, s);
-                g_trace.push_back(B200TraceRec{ "mul_cluster_kernel", t0, t1 });
-            }
             ctx->launches++;
             clustered = true;
         }
@@ -2120,34 +2096,6 @@ static int multiply_core(b200_ctx *ctx, int level, const u64 *a, int sa, const u
     return 0;
 }
 
-// b200_apply_galois_add through keyswitch_core: the target is sigma_g(c1) of in2 [item][2][k][n], dst = addend2 + apply_galois(in2)
-struct KsGalois
-{
-    const u64 *in2, *addend2; // addend2 == nullptr: no addend
-    u32 g, ginv;              // the Galois element and its inverse mod 2n
-};
-
-// b200_multiply_relin_sum through keyswitch_core: the batch is R outputs of m consecutive items; dst[r] = addend[r] +
-// sum_j (base_j + moddown(ks2_j)) over the items of output r (moddown_sum_kernel)
-struct KsSum
-{
-    const u64 *base;   // [item][2][k][n] c0 / c1 of each product, or nullptr where D is kept (keyswitch_core's D)
-    const u64 *addend; // [R][2][k][n] or nullptr; may be dst
-    long long R;
-    int m;
-};
-
-// b200_apply_galois_many and the BSGS linear transform through keyswitch_core: item i's target is sigma_{g_i}(c1) of tab[i].ct
-// with key list tab[i].key.  R == 0: each item's result goes to tab[i].dst (ksmoddown_galois_many_kernel); R > 0: the batch is
-// m R items, item j R + r a term of output r, and dst[r] = addend[r] + the sum of its terms (moddown_galois_sum_kernel).
-struct KsMany
-{
-    const B200GalItem *d_tab;           // [batch], device memory
-    const std::vector<B200GalItem> *tab; // the same table on the host: the key groups of the separate kernels' MAC
-    const u64 *addend;                  // R > 0: [R][2][k][n] or nullptr
-    long long R;
-};
-
 // moddown_sum_kernel's term split: R outputs give R n / EB CTAs.  Where those would not fill the GPU (the kernel's resident
 // CTAs per SM times the SM count), the m terms of each output are split into G <= m groups, so that R G n / EB CTAs do; the
 // G partial sums then go through a second launch of the same kernel without a key switch.
@@ -2173,21 +2121,25 @@ static int moddown_sum_groups(b200_ctx *ctx, long long R, int m)
     return (int)std::min<long long>(m, (capacity + ctas - 1) / ctas);
 }
 
-// ---- key switch core: target d (k rows per item, stride d_stride), key list; dst_c = base_c + moddown(acc_c) ----
-// D (FP64 levels only; base0 / base1 unused): the unscaled products of multiply_core's keep_D; base_c = scale(D_c), formed in
-// the mod-down kernel; dst is then [item][2][k][n]
-// gal (d, d_stride, base0 / base1 unused): the rotate-add of KsGalois.  The cluster kernel gathers sigma_g(c1) in its digit loads;
-// otherwise galois_kernel writes sigma_g(c1) alone to scratch for the separate kernels.  The mod-down gathers sigma_g(c0) and adds
-// the addend (ksmoddown_galois_add_kernel); dst is then [item][2][k][n]
-// sum (base0 / base1 unused): the multiply_relin sums of KsSum (moddown_sum_kernel, with D where given); dst is then
-// [sum->R][2][k][n]
-// many (d, key, base0 / base1 unused): the per-item elements and keys of KsMany.  The cluster kernel reads them from the table
-// (ks_cluster_galois_multi_kernel); otherwise galois_many_kernel writes the targets to scratch, and the MAC runs once per run
-// of consecutive items with one key.  dst is used by the sum mod-down only ([many->R][2][k][n])
-static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_stride, const u64 *key, const u64 *base0,
-                          long long base0_stride, const u64 *base1, long long base1_stride, u64 *dst,
-                          long long dst_stride, long long batch, cudaStream_t s, const u64 *D = nullptr,
-                          const KsGalois *gal = nullptr, const KsSum *sum = nullptr, const KsMany *many = nullptr)
+// What keyswitch_accumulate transforms, in one of three forms:
+//   rows:   k rows per item at d, item stride d_stride, with key list `key`;
+//   galois: g != 0: sigma_g(c1) of the ciphertexts d ([item][2][k][n]; ginv = g^-1 mod 2n), with key list `key`;
+//   table:  tab != nullptr: item i is sigma_{g_i}(c1) of tab[i].ct with key list tab[i].key; d_tab is the same table in
+//           device memory.
+struct KsTarget
+{
+    const u64 *d = nullptr;
+    long long d_stride = 0;
+    const u64 *key = nullptr;
+    u32 g = 0, ginv = 0;
+    const B200GalItem *d_tab = nullptr;
+    const std::vector<B200GalItem> *tab = nullptr;
+};
+
+// ---- key switch, all but the mod-down: ks2 [batch][2][k + 1][n] (coefficient form, canonical) = the inverse NTTs of the key
+// inner products of the target's digits, allocated in scr.  Each operation then launches its own mod-down of ks2. ----
+static int keyswitch_accumulate(b200_ctx *ctx, int level, const KsTarget &t, long long batch, Scratch &scr, cudaStream_t s,
+                                u64 **ks2_out)
 {
     if (!ctx->host->using_keyswitching || level < 1)
         return fail(B200_E_LOGIC, "keyswitching is not supported by the context");
@@ -2197,21 +2149,20 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
     const int k = L.k;
     const int Kkey = ctx->host->K;
     const int special = Kkey - 1;
-    Scratch scr(ctx, s);
     u64 *ks1 = nullptr, *ks2 = nullptr;
     int rc;
     if ((rc = scr.get((size_t)batch * 2 * (k + 1) * n, &ks2)))
         return rc;
-    if (gal)
-    {
-        d = gal->in2 + (long long)k * n;
-        d_stride = 2LL * k * n;
-    }
+    *ks2_out = ks2;
+    // the rows the digits are read from: the target's, or (galois form) the c1 rows of the ciphertexts
+    const u64 *d = t.g ? t.d + (long long)k * n : t.d;
+    long long d_stride = t.g ? 2LL * k * n : t.d_stride;
     bool clustered = false; // the forward NTTs, the inner product and the inverse NTTs ran as ks_cluster_kernel
 #ifndef B200_EMU_HEADER
     // all three in one kernel on the FP64 static path (mul_cluster.cu): the transformed digits and the accumulators stay in the
     // shared memory of a k-CTA cluster.  Taken where the launch fills the GPU (the rule of the 256/512 thread switch in
-    // launch_ntt and of the multiply's cluster); B200_KS_CLUSTER=0 selects the separate kernels below.
+    // launch_ntt and of the multiply's cluster); B200_KS_CLUSTER=0 selects the separate kernels below.  The galois forms gather
+    // sigma_g(c1) in the cluster kernel's digit loads.
     static const bool want_cluster = !(std::getenv("B200_KS_CLUSTER") && std::getenv("B200_KS_CLUSTER")[0] == '0');
     if (want_cluster && L.fp && ctx->logn <= 13 && k >= 2 && k <= 8 && ctx->ks_clusters[k] > 0 &&
         (long long)k * (k + 1) * batch > 2LL * ctx->sm_count)
@@ -2235,54 +2186,38 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
             job.fprimes = ctx->d_fp_primes;
             job.reduce_input = 1;
             job.items = batch;
-            cudaEvent_t t0 = nullptr, t1 = nullptr;
-            if (trace_on())
-            {
-                cudaEventCreate(&t0);
-                cudaEventCreate(&t1);
-                cudaEventRecord(t0, s);
-            }
-            const char *kname = many ? "ks_cluster_galois_multi_kernel" : gal ? "ks_cluster_galois_kernel" : "ks_cluster_kernel";
-            const int crc = many ? b200_ks_cluster_multi(ctx->logn, job, many->d_tab, Kkey, ks2, k, s)
-                                 : b200_ks_cluster(ctx->logn, job, d, d_stride, key, Kkey, ks2, k, gal ? gal->ginv : 0u, s);
+            const char *kname = t.tab ? "ks_cluster_galois_multi_kernel" : t.g ? "ks_cluster_galois_kernel" : "ks_cluster_kernel";
+            const int crc = traced_launch(kname, s, [&] {
+                return t.tab ? b200_ks_cluster_multi(ctx->logn, job, t.d_tab, Kkey, ks2, k, s)
+                             : b200_ks_cluster(ctx->logn, job, d, d_stride, t.key, Kkey, ks2, k, t.ginv, s);
+            });
             if (crc)
                 return fail(B200_E_CUDA, std::string(kname) + ": " + cudaGetErrorString((cudaError_t)crc));
-            if (t0)
-            {
-                cudaEventRecord(t1, s);
-                g_trace.push_back(B200TraceRec{ kname, t0, t1 });
-            }
             ctx->launches++;
             clustered = true;
         }
     }
 #endif
-    if (!clustered && (rc = scr.get((size_t)batch * (k + 1) * k * n, &ks1)))
+    if (clustered)
+        return 0;
+    if ((rc = scr.get((size_t)batch * (k + 1) * k * n, &ks1)))
         return rc;
-    if (!clustered && gal)
+    // the galois forms' targets, written to scratch for the digit NTTs
+    if (t.g || t.tab)
     {
         u64 *sc1 = nullptr;
         if ((rc = scr.get((size_t)batch * k * n, &sc1)))
             return rc;
         const long long total = batch * k * n;
-        B200_LAUNCH(galois_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, gal->in2, (u64 *)nullptr, sc1, ctx->logn, gal->g,
-                    total);
+        if (t.tab)
+            B200_LAUNCH(galois_many_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, t.d_tab, sc1, ctx->logn, total);
+        else
+            B200_LAUNCH(galois_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, t.d, (u64 *)nullptr, sc1, ctx->logn, t.g,
+                        total);
         ctx->launches++;
         d = sc1;
         d_stride = (long long)k * n;
     }
-    if (!clustered && many)
-    {
-        u64 *sc1 = nullptr;
-        if ((rc = scr.get((size_t)batch * k * n, &sc1)))
-            return rc;
-        const long long total = batch * k * n;
-        B200_LAUNCH(galois_many_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, many->d_tab, sc1, ctx->logn, total);
-        ctx->launches++;
-        d = sc1;
-        d_stride = (long long)k * n;
-    }
-    if (!clustered)
     {
         std::vector<int> prime;
         std::vector<long long> so, dof;
@@ -2299,13 +2234,14 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         if ((rc = launch_ntt<true>(ctx, jd, d, d_stride, ks1, (long long)(k + 1) * k * n, batch, 1, s)))
             return rc;
     }
-    // the MAC's runs of items with one key: [i0, i0 + cnt) with key `key` (many: the runs of equal tab[i].key)
-    for (long long i0 = 0, cnt = batch; !clustered && i0 < batch; i0 += cnt)
+    // the MAC's runs of items with one key: [i0, i0 + cnt) with key `key` (table form: the runs of equal tab[i].key)
+    for (long long i0 = 0, cnt = batch; i0 < batch; i0 += cnt)
     {
-        if (many)
+        const u64 *key = t.key;
+        if (t.tab)
         {
-            key = (*many->tab)[i0].key;
-            for (cnt = 1; i0 + cnt < batch && (*many->tab)[i0 + cnt].key == key; cnt++)
+            key = (*t.tab)[i0].key;
+            for (cnt = 1; i0 + cnt < batch && (*t.tab)[i0 + cnt].key == key; cnt++)
                 ;
         }
         const u64 *ks1g = ks1 + i0 * (k + 1) * k * n;
@@ -2317,29 +2253,13 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         static const bool want_tma = !(std::getenv("B200_KSMAC_TMA") && std::getenv("B200_KSMAC_TMA")[0] == '0');
         if (want_tma && b200_ksmac_tma_supported(n, k))
         {
-            if (trace_on())
-                g_trace_name = "ksmac_tma_kernel";
-            cudaEvent_t t0 = nullptr, t1 = nullptr;
-            if (trace_on())
-            {
-                cudaEventCreate(&t0);
-                cudaEventCreate(&t1);
-                cudaEventRecord(t0, s);
-            }
-            const int rc2 = b200_ksmac_tma(k, L.fp ? 1 : 0, ctx->d_primes, ctx->d_fp_primes, special, Kkey, ks1g, key, ks2g, n, cnt,
-                                           ctx->sm_count, s);
+            const int rc2 = traced_launch("ksmac_tma_kernel", s, [&] {
+                return b200_ksmac_tma(k, L.fp ? 1 : 0, ctx->d_primes, ctx->d_fp_primes, special, Kkey, ks1g, key, ks2g, n, cnt,
+                                      ctx->sm_count, s);
+            });
             if (rc2 > 0)
                 return fail(B200_E_CUDA, std::string("ksmac_tma_kernel: ") + cudaGetErrorString((cudaError_t)rc2));
-            if (rc2 == 0)
-            {
-                done = true;
-                if (t0)
-                {
-                    cudaEventRecord(t1, s);
-                    g_trace.push_back(B200TraceRec{ "ksmac_tma_kernel", t0, t1 });
-                    g_trace_name = nullptr;
-                }
-            }
+            done = rc2 == 0;
         }
 #endif
         if (done)
@@ -2358,101 +2278,40 @@ static int keyswitch_core(b200_ctx *ctx, int level, const u64 *d, long long d_st
         }
         ctx->launches++;
     }
-    if (!clustered)
-    {
-        std::vector<int> prime;
-        for (int comp = 0; comp < 2; comp++)
-            for (int I = 0; I <= k; I++)
-                prime.push_back(I < k ? Lh.q_idx[I] : special);
-        JobDesc jd;
-        if ((rc = dense_job(ctx, "ks2:" + std::to_string(level), prime, &jd)))
-            return rc;
-        if ((rc = launch_ntt<false>(ctx, jd, ks2, 2LL * (k + 1) * n, ks2, 2LL * (k + 1) * n, batch, 0, s)))
-            return rc;
-    }
-    if (sum)
-    {
-        // the SCALE variant exists up to B200_MR_SUM_SCALE_MAX_K residues (multiply_relin_sum_one keeps D only there)
-        int G = 1;
-        const long long R = sum->R;
-        u64 *part = nullptr;
-        auto launch = [&](auto kk, auto scale) -> int {
-            constexpr int KK = decltype(kk)::value;
-            constexpr bool SC = decltype(scale)::value && KK <= B200_MR_SUM_SCALE_MAX_K;
-            G = moddown_sum_groups<KK, SC>(ctx, R, sum->m);
-            int rc2;
-            if (G > 1 && (rc2 = scr.get((size_t)R * G * 2 * k * n, &part)))
-                return rc2;
-            const long long total = R * G * 2 * (n >> 1);
-            void (*k1)(const ScaleFpC<KK>, const PrimeDev *, int, const u64 *, const u64 *, const u64 *, const u64 *, const u64 *, u64 *,
-                       int, int, long long, long long) = moddown_sum_kernel<KK, SC>;
-#ifndef B200_EMU_HEADER
-            if (trace_on())
-                g_trace_name = "moddown_sum_kernel";
-#endif
-            B200_LAUNCH(k1, blocks_for(total, EB), EB, 0, s, SC ? make_scale_fpc<KK>(ctx, level) : ScaleFpC<KK>{}, ctx->d_primes,
-                        special, ctx->d_inv_qsp, D, sum->base, ks2, G > 1 ? nullptr : sum->addend, G > 1 ? part : dst, sum->m, G, n, total);
-            ctx->launches++;
-            if (G > 1)
-            {
-                // the G partial sums of each output, without a key switch
-                const long long total2 = R * 2 * (n >> 1);
-                k1 = moddown_sum_kernel<KK, false>;
-#ifndef B200_EMU_HEADER
-                if (trace_on())
-                    g_trace_name = "moddown_sum_kernel";
-#endif
-                B200_LAUNCH(k1, blocks_for(total2, EB), EB, 0, s, ScaleFpC<KK>{}, ctx->d_primes, special, ctx->d_inv_qsp,
-                            (const u64 *)nullptr, (const u64 *)part, (const u64 *)nullptr, sum->addend, dst, G, 1, n, total2);
-                ctx->launches++;
-            }
-            return 0;
-        };
-        if (D && k > B200_MR_SUM_SCALE_MAX_K)
-            return fail(B200_E_INVALID, "moddown_sum_kernel: no scaling variant at this residue count");
-        if (D)
-        {
-            DISPATCH_K(k, if ((rc = launch(std::integral_constant<int, KK>(), std::true_type()))) return rc);
-        }
-        else
-        {
-            DISPATCH_K(k, if ((rc = launch(std::integral_constant<int, KK>(), std::false_type()))) return rc);
-        }
-    }
-    else
-    {
-        const long long total = batch * 2 * (n >> 1);
-        if (many && many->R > 0)
-        {
-            const long long R = many->R, total2 = R * 2 * (n >> 1);
-            DISPATCH_K(k, B200_LAUNCH(moddown_galois_sum_kernel<KK>, blocks_for(total2, EB), EB, 0, s, ctx->d_primes, special,
-                                      ctx->d_inv_qsp, ks2, many->d_tab, many->addend, dst, (int)(batch / R), R, ctx->logn, total2));
-        }
-        else if (many)
-        {
-            DISPATCH_K(k, B200_LAUNCH(ksmoddown_galois_many_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special,
-                                      ctx->d_inv_qsp, ks2, many->d_tab, ctx->logn, total));
-        }
-        else if (gal)
-        {
-            DISPATCH_K(k, B200_LAUNCH(ksmoddown_galois_add_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special,
-                                      ctx->d_inv_qsp, ks2, gal->in2, gal->addend2, dst, ctx->logn, gal->ginv, total));
-        }
-        else if (D)
-        {
-            DISPATCH_K(k, B200_LAUNCH(scale_moddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, make_scale_fpc<KK>(ctx, level),
-                                      ctx->d_primes, special, ctx->d_inv_qsp, D, ks2, dst, n, total));
-        }
-        else
-        {
-            DISPATCH_K(k, B200_LAUNCH(ksmoddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special, ctx->d_inv_qsp, ks2,
-                                                                                    base0, base0_stride, base1, base1_stride,
-                                                                                    dst, dst_stride, n, total));
-        }
-        ctx->launches++;
-    }
+    std::vector<int> prime;
+    for (int comp = 0; comp < 2; comp++)
+        for (int I = 0; I <= k; I++)
+            prime.push_back(I < k ? Lh.q_idx[I] : special);
+    JobDesc jd;
+    if ((rc = dense_job(ctx, "ks2:" + std::to_string(level), prime, &jd)))
+        return rc;
+    return launch_ntt<false>(ctx, jd, ks2, 2LL * (k + 1) * n, ks2, 2LL * (k + 1) * n, batch, 0, s);
+}
+
+// dst_c = base_c + moddown(ks2_c) for the components c = 0, 1 (ksmoddown_kernel_v2): base_c at base0 / base1 with item stride
+// base_stride (nullptr: zero), dst [batch][2][k][n]
+static int ksmoddown(b200_ctx *ctx, int level, const u64 *ks2, const u64 *base0, const u64 *base1, long long base_stride, u64 *dst,
+                     long long batch, cudaStream_t s)
+{
+    const long long n = (long long)ctx->n;
+    const int k = ctx->levels[level].k;
+    const long long total = batch * 2 * (n >> 1);
+    DISPATCH_K(k, B200_LAUNCH(ksmoddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, ctx->host->K - 1, ctx->d_inv_qsp,
+                              ks2, base0, base_stride, base1, base_stride, dst, 2LL * k * n, n, total));
+    ctx->launches++;
     CU_TRY(cudaGetLastError());
     return 0;
+}
+
+// Whether multiply+relinearize keeps the unscaled products D (3R rows per item, R = k + |Bsk|) and scales them inside the
+// mod-down (scale_moddown_kernel_v2; moddown_sum_kernel<K, true> for sums): on FP64 levels where D beside the key switch's
+// scratch (at most k(k + 1) + 2(k + 1) rows) stays within the multiply's own ext + D (7R), i.e. (k + 1)(k + 2) <= 4R; sums
+// also need k <= B200_MR_SUM_SCALE_MAX_K.  Elsewhere (k = 7, 8 of the n = 16384 chain) c0 / c1 are scaled separately, which
+// keeps the peak scratch where the multiply alone has it.
+static bool mr_keeps_D(const LevelDev &L, bool sum)
+{
+    const int k = L.k, R = k + L.nBsk;
+    return L.fp && (k + 1) * (k + 2) <= 4 * R && (!sum || k <= B200_MR_SUM_SCALE_MAX_K);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -3155,8 +3014,13 @@ int b200_relinearize(b200_ctx *ctx, int level, const uint64_t *in3, const uint64
     const long long n = (long long)ctx->n;
     const int k = ctx->levels[level].k;
     const u64 *c = (const u64 *)in3;
-    return keyswitch_core(ctx, level, c + 2LL * k * n, 3LL * k * n, (const u64 *)relin_key, c, 3LL * k * n, c + (long long)k * n,
-                          3LL * k * n, (u64 *)out2, 2LL * k * n, (long long)batch, (cudaStream_t)stream);
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    u64 *ks2 = nullptr;
+    if ((rc = keyswitch_accumulate(ctx, level, KsTarget{ c + 2LL * k * n, 3LL * k * n, (const u64 *)relin_key }, (long long)batch, scr,
+                                   s, &ks2)))
+        return rc;
+    return ksmoddown(ctx, level, ks2, c, c + (long long)k * n, 3LL * k * n, (u64 *)out2, (long long)batch, s);
 }
 
 static int multiply_relin_one(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, const uint64_t *relin_key,
@@ -3175,28 +3039,32 @@ static int multiply_relin_one(b200_ctx *ctx, int level, const uint64_t *a, const
     const int k = L.k, R = k + L.nBsk;
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
-    u64 *c2 = nullptr, *D = nullptr;
+    u64 *c2 = nullptr, *D = nullptr, *ks2 = nullptr;
     if ((rc = scr.get((size_t)batch * k * n, &c2)))
         return rc;
     u64 *o = (u64 *)out2;
-    // FP64 levels: c0, c1 are scaled inside the key switch's mod-down (scale_moddown_kernel_v2), from the products D kept
-    // here, instead of going through out2 and back.  D (3R rows per item) then lives beside the key switch's scratch (at most
-    // k(k + 1) + 2(k + 1) rows), which stays within the multiply's own ext + D (7R) while (k + 1)(k + 2) <= 4R; above that
-    // (k = 7, 8 of the n = 16384 chain) the separate scale keeps the peak scratch where it was.
-    if (L.fp && (k + 1) * (k + 2) <= 4 * R)
+    const KsTarget target{ c2, (long long)k * n, (const u64 *)relin_key };
+    // c0, c1 scaled inside the key switch's mod-down (scale_moddown_kernel_v2), from the products D kept here, instead of
+    // going through out2 and back
+    if (mr_keeps_D(L, false))
     {
         if ((rc = scr.get((size_t)batch * 3 * R * n, &D)))
             return rc;
-        if ((rc = multiply_core(ctx, level, (const u64 *)a, 2, (const u64 *)b, 2, false, nullptr, 2, c2, (long long)batch, s, D)))
+        if ((rc = multiply_core(ctx, level, (const u64 *)a, 2, (const u64 *)b, 2, false, nullptr, 2, c2, (long long)batch, s, D)) ||
+            (rc = keyswitch_accumulate(ctx, level, target, (long long)batch, scr, s, &ks2)))
             return rc;
-        return keyswitch_core(ctx, level, c2, (long long)k * n, (const u64 *)relin_key, nullptr, 0, nullptr, 0, o, 2LL * k * n,
-                              (long long)batch, s, D);
+        const long long total = (long long)batch * 2 * (n >> 1);
+        DISPATCH_K(k, B200_LAUNCH(scale_moddown_kernel_v2<KK>, blocks_for(total, EB), EB, 0, s, make_scale_fpc<KK>(ctx, level),
+                                  ctx->d_primes, ctx->host->K - 1, ctx->d_inv_qsp, D, ks2, o, n, total));
+        ctx->launches++;
+        CU_TRY(cudaGetLastError());
+        return 0;
     }
     // c0,c1 go straight into out2; c2 into scratch
-    if ((rc = multiply_core(ctx, level, (const u64 *)a, 2, (const u64 *)b, 2, false, o, 2, c2, (long long)batch, s)))
+    if ((rc = multiply_core(ctx, level, (const u64 *)a, 2, (const u64 *)b, 2, false, o, 2, c2, (long long)batch, s)) ||
+        (rc = keyswitch_accumulate(ctx, level, target, (long long)batch, scr, s, &ks2)))
         return rc;
-    return keyswitch_core(ctx, level, c2, (long long)k * n, (const u64 *)relin_key, o, 2LL * k * n, o + (long long)k * n,
-                          2LL * k * n, o, 2LL * k * n, (long long)batch, s);
+    return ksmoddown(ctx, level, ks2, o, o + (long long)k * n, 2LL * k * n, o, (long long)batch, s);
 }
 
 int b200_multiply_relin(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, const uint64_t *relin_key,
@@ -3225,35 +3093,71 @@ int b200_multiply_relin(b200_ctx *ctx, int level, const uint64_t *a, const uint6
 }
 
 // out[r] = addend[r] + sum_{j < m} relinearize(multiply(a[r][j], b[r][j])) for r < rows: multiply_relin_one over the rows m
-// items with keyswitch_core's sum mod-down (moddown_sum_kernel) in place of the per-item one.  D is kept on multiply_relin_one's
-// rule; otherwise c0 / c1 of every product go to scratch ([item][2][k][n]) and the mod-down sums them from there.
+// items with a sum mod-down (moddown_sum_kernel) in place of the per-item one.  D is kept on mr_keeps_D's rule; otherwise
+// c0 / c1 of every product go to scratch ([item][2][k][n]) and the mod-down sums them from there.  addend ([rows][2][k][n] or
+// nullptr) may be out2.
 static int multiply_relin_sum_one(b200_ctx *ctx, int level, const u64 *a, const u64 *b, const u64 *relin_key, int m, u64 *out2,
                                   long long rows, const u64 *addend, cudaStream_t s)
 {
     const long long n = (long long)ctx->n;
     const LevelDev &L = ctx->levels[level];
     const int k = L.k, R = k + L.nBsk;
+    const int special = ctx->host->K - 1;
     const long long items = rows * m;
+    const bool keepD = mr_keeps_D(L, true);
     Scratch scr(ctx, s);
-    u64 *c2 = nullptr, *D = nullptr, *c01 = nullptr;
+    u64 *c2 = nullptr, *D = nullptr, *c01 = nullptr, *ks2 = nullptr;
     int rc;
-    if ((rc = scr.get((size_t)items * k * n, &c2)))
+    if ((rc = scr.get((size_t)items * k * n, &c2)) || (rc = scr.get((size_t)items * (keepD ? 3 * R : 2 * k) * n, keepD ? &D : &c01)) ||
+        (rc = multiply_core(ctx, level, a, 2, b, 2, false, c01, 2, c2, items, s, D)) ||
+        (rc = keyswitch_accumulate(ctx, level, KsTarget{ c2, (long long)k * n, relin_key }, items, scr, s, &ks2)))
         return rc;
-    if (L.fp && (k + 1) * (k + 2) <= 4 * R && k <= B200_MR_SUM_SCALE_MAX_K)
+    // the term split of moddown_sum_groups: G > 1 partial sums per output go to part, then through a second launch without a
+    // key switch.  The SCALE variant exists up to B200_MR_SUM_SCALE_MAX_K residues.
+    auto launch = [&](auto kk, auto scale) -> int {
+        constexpr int KK = decltype(kk)::value;
+        constexpr bool SC = decltype(scale)::value && KK <= B200_MR_SUM_SCALE_MAX_K;
+        const int G = moddown_sum_groups<KK, SC>(ctx, rows, m);
+        u64 *part = nullptr;
+        int rc2;
+        if (G > 1 && (rc2 = scr.get((size_t)rows * G * 2 * k * n, &part)))
+            return rc2;
+        const long long total = rows * G * 2 * (n >> 1);
+        void (*k1)(const ScaleFpC<KK>, const PrimeDev *, int, const u64 *, const u64 *, const u64 *, const u64 *, const u64 *, u64 *,
+                   int, int, long long, long long) = moddown_sum_kernel<KK, SC>;
+#ifndef B200_EMU_HEADER
+        if (trace_on())
+            g_trace_name = "moddown_sum_kernel";
+#endif
+        B200_LAUNCH(k1, blocks_for(total, EB), EB, 0, s, SC ? make_scale_fpc<KK>(ctx, level) : ScaleFpC<KK>{}, ctx->d_primes, special,
+                    ctx->d_inv_qsp, D, c01, ks2, G > 1 ? nullptr : addend, G > 1 ? part : out2, m, G, n, total);
+        ctx->launches++;
+        if (G > 1)
+        {
+            const long long total2 = rows * 2 * (n >> 1);
+            k1 = moddown_sum_kernel<KK, false>;
+#ifndef B200_EMU_HEADER
+            if (trace_on())
+                g_trace_name = "moddown_sum_kernel";
+#endif
+            B200_LAUNCH(k1, blocks_for(total2, EB), EB, 0, s, ScaleFpC<KK>{}, ctx->d_primes, special, ctx->d_inv_qsp, (const u64 *)nullptr,
+                        (const u64 *)part, (const u64 *)nullptr, addend, out2, G, 1, n, total2);
+            ctx->launches++;
+        }
+        return 0;
+    };
+    if (keepD && k > B200_MR_SUM_SCALE_MAX_K)
+        return fail(B200_E_INVALID, "moddown_sum_kernel: no scaling variant at this residue count");
+    if (keepD)
     {
-        const KsSum sum{ nullptr, addend, rows, m };
-        if ((rc = scr.get((size_t)items * 3 * R * n, &D)))
-            return rc;
-        if ((rc = multiply_core(ctx, level, a, 2, b, 2, false, nullptr, 2, c2, items, s, D)))
-            return rc;
-        return keyswitch_core(ctx, level, c2, (long long)k * n, relin_key, nullptr, 0, nullptr, 0, out2, 0, items, s, D, nullptr, &sum);
+        DISPATCH_K(k, if ((rc = launch(std::integral_constant<int, KK>(), std::true_type()))) return rc);
     }
-    if ((rc = scr.get((size_t)items * 2 * k * n, &c01)))
-        return rc;
-    if ((rc = multiply_core(ctx, level, a, 2, b, 2, false, c01, 2, c2, items, s)))
-        return rc;
-    const KsSum sum{ c01, addend, rows, m };
-    return keyswitch_core(ctx, level, c2, (long long)k * n, relin_key, nullptr, 0, nullptr, 0, out2, 0, items, s, nullptr, nullptr, &sum);
+    else
+    {
+        DISPATCH_K(k, if ((rc = launch(std::integral_constant<int, KK>(), std::false_type()))) return rc);
+    }
+    CU_TRY(cudaGetLastError());
+    return 0;
 }
 
 int b200_multiply_relin_sum(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, const uint64_t *relin_key, uint64_t m,
@@ -3287,8 +3191,7 @@ int b200_multiply_relin_sum(b200_ctx *ctx, int level, const uint64_t *a, const u
     cudaStream_t s = (cudaStream_t)stream;
     // scratch of one term at its peak: c2 with D (or c0 / c1) held, plus the larger of the multiply's ext + D and the key
     // switch's ks1 + ks2
-    const bool keepD = L.fp && (k + 1) * (k + 2) <= 4 * R && k <= B200_MR_SUM_SCALE_MAX_K;
-    const size_t held = (size_t)k + (keepD ? 3 * R : 2 * k);
+    const size_t held = (size_t)k + (mr_keeps_D(L, true) ? 3 * R : 2 * k);
     const size_t term_bytes = (held + std::max<size_t>((size_t)7 * R, (size_t)(k + 1) * (k + 2))) * n * sizeof(u64);
     uint64_t cap = 1ull << 30;
     if (const char *e = std::getenv("B200_MR_SUM_SCRATCH"))
@@ -3318,6 +3221,66 @@ int b200_multiply_relin_sum(b200_ctx *ctx, int level, const uint64_t *a, const u
     return rc;
 }
 
+// g^-1 mod 2n = g^(n-1): the odd residues mod 2n form a group of order n
+static u32 galois_inverse(u64 n, u32 g)
+{
+    const u64 m2 = 2 * n;
+    u64 ginv = 1, base = g;
+    for (u64 e = n - 1; e; e >>= 1, base = base * base % m2)
+        if (e & 1)
+            ginv = ginv * base % m2;
+    return (u32)ginv;
+}
+
+// a host table copied into stream-ordered scratch (the copy from pageable memory is staged before cudaMemcpyAsync returns)
+static int upload_table(Scratch &scr, const void *host, size_t bytes, cudaStream_t s, const void **out)
+{
+    u64 *p = nullptr;
+    int rc;
+    if ((rc = scr.get((bytes + 7) / 8, &p)))
+        return rc;
+    CU_TRY(cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, s));
+    *out = p;
+    return 0;
+}
+
+// A key switch with a Galois element and a key list per item: item i is apply_galois(tab[i].ct, tab[i].g) with key tab[i].key.
+// R == 0: item i's result goes to tab[i].dst (ksmoddown_galois_many_kernel).  R > 0: the batch is m R terms, item j R + r a
+// term of output r, and dst[r] = addend[r] + the sum of its terms in term order (moddown_galois_sum_kernel; addend
+// [R][2][k][n] or nullptr, may be dst).
+static int galois_table_keyswitch(b200_ctx *ctx, int level, const std::vector<B200GalItem> &tab, long long R, const u64 *addend,
+                                  u64 *dst, cudaStream_t s)
+{
+    const long long n = (long long)ctx->n, batch = (long long)tab.size();
+    const int k = ctx->levels[level].k, special = ctx->host->K - 1;
+    Scratch scr(ctx, s);
+    const B200GalItem *d_tab = nullptr;
+    u64 *ks2 = nullptr;
+    int rc;
+    if ((rc = upload_table(scr, tab.data(), tab.size() * sizeof(B200GalItem), s, (const void **)&d_tab)))
+        return rc;
+    KsTarget target;
+    target.d_tab = d_tab;
+    target.tab = &tab;
+    if ((rc = keyswitch_accumulate(ctx, level, target, batch, scr, s, &ks2)))
+        return rc;
+    if (R > 0)
+    {
+        const long long total = R * 2 * (n >> 1);
+        DISPATCH_K(k, B200_LAUNCH(moddown_galois_sum_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special, ctx->d_inv_qsp,
+                                  ks2, d_tab, addend, dst, (int)(batch / R), R, ctx->logn, total));
+    }
+    else
+    {
+        const long long total = batch * 2 * (n >> 1);
+        DISPATCH_K(k, B200_LAUNCH(ksmoddown_galois_many_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, special,
+                                  ctx->d_inv_qsp, ks2, d_tab, ctx->logn, total));
+    }
+    ctx->launches++;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
 int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
                       uint64_t *out2, uint64_t batch, void *stream)
 {
@@ -3338,7 +3301,7 @@ int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t ga
     const int k = L.k;
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
-    u64 *tmp = nullptr;
+    u64 *tmp = nullptr, *ks2 = nullptr;
     if ((rc = scr.get((size_t)batch * k * n, &tmp)))
         return rc;
     const long long total = (long long)batch * 2 * k * n;
@@ -3346,8 +3309,10 @@ int b200_apply_galois(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t ga
                                                        galois_elt, total);
     ctx->launches++;
     u64 *o = (u64 *)out2;
-    return keyswitch_core(ctx, level, tmp, (long long)k * n, (const u64 *)galois_key, o, 2LL * k * n, nullptr, 0, o,
-                          2LL * k * n, (long long)batch, s);
+    if ((rc = keyswitch_accumulate(ctx, level, KsTarget{ tmp, (long long)k * n, (const u64 *)galois_key }, (long long)batch, scr, s,
+                                   &ks2)))
+        return rc;
+    return ksmoddown(ctx, level, ks2, o, nullptr, 2LL * k * n, o, (long long)batch, s);
 }
 
 int b200_apply_galois_add(b200_ctx *ctx, int level, const uint64_t *in2, uint32_t galois_elt, const uint64_t *galois_key,
@@ -3372,37 +3337,20 @@ int b200_apply_galois_add(b200_ctx *ctx, int level, const uint64_t *in2, uint32_
     if (batch == 0)
         return 0;
     CU_TRY(cudaSetDevice(ctx->device));
-    // g^-1 mod 2n = g^(n-1): the odd residues mod 2n form a group of order n
-    const u64 m2 = 2 * (u64)ctx->n;
-    u64 ginv = 1, base = galois_elt;
-    for (u64 e = ctx->n - 1; e; e >>= 1, base = base * base % m2)
-        if (e & 1)
-            ginv = ginv * base % m2;
-    const KsGalois gal{ (const u64 *)in2, (const u64 *)addend2, galois_elt, (u32)ginv };
-    return keyswitch_core(ctx, level, nullptr, 0, (const u64 *)galois_key, nullptr, 0, nullptr, 0, (u64 *)out2, 0, (long long)batch,
-                          (cudaStream_t)stream, nullptr, &gal);
-}
-
-// g^-1 mod 2n = g^(n-1): the odd residues mod 2n form a group of order n
-static u32 galois_inverse(u64 n, u32 g)
-{
-    const u64 m2 = 2 * n;
-    u64 ginv = 1, base = g;
-    for (u64 e = n - 1; e; e >>= 1, base = base * base % m2)
-        if (e & 1)
-            ginv = ginv * base % m2;
-    return (u32)ginv;
-}
-
-// a host table copied into stream-ordered scratch (the copy from pageable memory is staged before cudaMemcpyAsync returns)
-static int upload_table(Scratch &scr, const void *host, size_t bytes, cudaStream_t s, const void **out)
-{
-    u64 *p = nullptr;
-    int rc;
-    if ((rc = scr.get((bytes + 7) / 8, &p)))
+    const int k = ctx->levels[level].k;
+    const u32 ginv = galois_inverse(ctx->n, galois_elt);
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    u64 *ks2 = nullptr;
+    if ((rc = keyswitch_accumulate(ctx, level, KsTarget{ (const u64 *)in2, 0, (const u64 *)galois_key, galois_elt, ginv },
+                                   (long long)batch, scr, s, &ks2)))
         return rc;
-    CU_TRY(cudaMemcpyAsync(p, host, bytes, cudaMemcpyHostToDevice, s));
-    *out = p;
+    // dst = addend2 + sigma_g(c0) + moddown(ks2), sigma_g(c0) gathered in the mod-down
+    const long long total = (long long)batch * 2 * (ctx->n >> 1);
+    DISPATCH_K(k, B200_LAUNCH(ksmoddown_galois_add_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, ctx->host->K - 1,
+                              ctx->d_inv_qsp, ks2, (const u64 *)in2, (const u64 *)addend2, (u64 *)out2, ctx->logn, ginv, total));
+    ctx->launches++;
+    CU_TRY(cudaGetLastError());
     return 0;
 }
 
@@ -3433,18 +3381,11 @@ int b200_apply_galois_many(b200_ctx *ctx, int level, const uint64_t *in2, const 
             return fail(B200_E_INVALID, "apply_galois_many: out overlaps in");
     }
     CU_TRY(cudaSetDevice(ctx->device));
-    cudaStream_t s = (cudaStream_t)stream;
     std::vector<B200GalItem> tab(batch);
     for (uint64_t i = 0; i < batch; i++)
         tab[i] = B200GalItem{ (const u64 *)in2 + (src_idx ? src_idx[i] : i) * w, (const u64 *)keys[i], (u64 *)out2 + i * w, elts[i],
                               galois_inverse(ctx->n, elts[i]) };
-    Scratch scr(ctx, s);
-    const B200GalItem *d_tab = nullptr;
-    if ((rc = upload_table(scr, tab.data(), tab.size() * sizeof(B200GalItem), s, (const void **)&d_tab)))
-        return rc;
-    const KsMany many{ d_tab, &tab, nullptr, 0 };
-    return keyswitch_core(ctx, level, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, (long long)batch, s, nullptr, nullptr,
-                          nullptr, &many);
+    return galois_table_keyswitch(ctx, level, tab, 0, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 // plain [pb][n] -> out [pb][k][n]: each plaintext lifted to the level's residues and put in NTT form.  monomial != 0 gives
@@ -3705,12 +3646,7 @@ int b200_linear_transform(b200_ctx *ctx, int level, const uint64_t *cts, uint64_
                     for (long long v = 0; v < Vc; v++)
                         tab.push_back(B200GalItem{ ct + v * w, (const u64 *)keys[j - 1], X + (j * Vc + v) * w, elts[j - 1],
                                                    galois_inverse(ctx->n, elts[j - 1]) });
-            const B200GalItem *d_tab = nullptr;
-            if ((rc = upload_table(scr, tab.data(), tab.size() * sizeof(B200GalItem), s, (const void **)&d_tab)))
-                return rc;
-            const KsMany many{ d_tab, &tab, nullptr, 0 };
-            if ((rc = keyswitch_core(ctx, level, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, (long long)tab.size(), s, nullptr,
-                                     nullptr, nullptr, &many)))
+            if ((rc = galois_table_keyswitch(ctx, level, tab, 0, nullptr, nullptr, s)))
                 return rc;
         }
         // forward NTT of the rotated copies: one launch per run of consecutive used steps (one run when every step is used)
@@ -3747,12 +3683,7 @@ int b200_linear_transform(b200_ctx *ctx, int level, const uint64_t *cts, uint64_
                 for (long long v = 0; v < Vc; v++)
                     tab.push_back(B200GalItem{ inner + (g * Vc + v) * w, (const u64 *)keys[e], nullptr, elts[e], galois_inverse(ctx->n, elts[e]) });
             }
-        const B200GalItem *d_tab = nullptr;
-        if ((rc = upload_table(scr, tab.data(), tab.size() * sizeof(B200GalItem), s, (const void **)&d_tab)))
-            return rc;
-        const KsMany many{ d_tab, &tab, ug[0] ? inner : nullptr, Vc };
-        if ((rc = keyswitch_core(ctx, level, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, o, 0, (long long)tab.size(), s, nullptr, nullptr,
-                                 nullptr, &many)))
+        if ((rc = galois_table_keyswitch(ctx, level, tab, Vc, ug[0] ? inner : nullptr, o, s)))
             return rc;
     }
     CU_TRY(cudaGetLastError());

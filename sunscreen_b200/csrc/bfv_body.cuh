@@ -306,34 +306,6 @@ B200_HD void ksmac_coeff(const PrimeDev &P, const u64 *__restrict__ ops, long lo
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// key switch mod-down: acc rows [K data residues + 1 special] (coefficient form, canonical) added into ct poly
-//   s = [acc_sp + floor(q_sp/2)]_{q_sp};  ct_i += (acc_i - [s]_{q_i} + [floor(q_sp/2)]_{q_i}) * q_sp^-1   (mod q_i)
-// `base`: optional polynomial to add (nullptr = 0); result written to dst rows.
-// ---------------------------------------------------------------------------------------------------------
-template <int K>
-B200_HD void ksmoddown_coeff(const PrimeDev *__restrict__ q /*[K]*/, const PrimeDev &SP,
-                             const u64 *__restrict__ inv_qsp /*[2K] shoup*/, const u64 *__restrict__ acc, long long n,
-                             const u64 *__restrict__ base, u64 *__restrict__ dst, long long c)
-{
-    const u64 half = SP.p >> 1;
-    u64 s = acc[K * n + c] + half;
-    s = s >= SP.p ? s - SP.p : s;
-#pragma unroll
-    for (int i = 0; i < K; i++)
-    {
-        const PrimeDev Q = ld_prime(&q[i]);
-        const u64 r = barrett64(s, Q.p, Q.r1);
-        const u64 h = barrett64(half, Q.p, Q.r1);
-        // (a - r + h) mod q, computed without underflow: a + (q - r) + h < 3q
-        u64 v = acc[i * n + c] + (Q.p - r) + h;
-        v = shoup_mul(v, B200_LDG(&inv_qsp[2 * i]), B200_LDG(&inv_qsp[2 * i + 1]), Q.p);
-        if (base)
-            v = add_mod(v, base[i * n + c], Q.p);
-        dst[i * n + c] = v;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
 // divide-and-round by the last prime (BFV mod switch): rows [K] -> [K-1]
 // ---------------------------------------------------------------------------------------------------------
 template <int K>

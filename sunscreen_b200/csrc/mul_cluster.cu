@@ -15,7 +15,7 @@
 //
 // ks_cluster_kernel gives the key switch the same treatment: a k-CTA cluster per (item, key residue I) transforms the k digits
 // mod p_I, forms the two inner products with the key and transforms them back, instead of the ks1 NTT, the MAC and the ks2 NTT
-// of keyswitch_core.  Its hand-offs are canonical as well: the digits before the products (the words of ks1), the accumulators
+// of keyswitch_accumulate.  Its hand-offs are canonical as well: the digits before the products (the words of ks1), the accumulators
 // (the words of ks2, formed by the FP64 branch of ksmac_tma_kernel), so every word and every renorm bound equals the separate path's.
 #include "mul_cluster.h"
 #include "ntt_fp_body.cuh"

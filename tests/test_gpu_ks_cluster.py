@@ -1,10 +1,10 @@
 """The fused key switch (ks_cluster_kernel, sunscreen_b200/csrc/mul_cluster.cu) against the unmodified reference, on either
 side of its dispatch rule, and the launch trace that shows which path ran (pytest -m gpu).
 
-keyswitch_core runs the forward NTTs of the digits, the inner product with the key and the inverse NTTs as one k-CTA
+keyswitch_accumulate runs the forward NTTs of the digits, the inner product with the key and the inverse NTTs as one k-CTA
 cluster kernel for levels on the FP64 path at n <= 8192 with 2 <= k <= 8 when the launch fills the GPU:
 k (k + 1) * batch > 2 * sm_count.  Below that, at k = 1, at n = 16384 and with B200_KS_CLUSTER=0 the separate kernels run.
-relinearize, multiply_relin and apply_galois all go through keyswitch_core; every output word is compared with the
+relinearize, multiply_relin and apply_galois all go through keyswitch_accumulate; every output word is compared with the
 reference."""
 import os
 import re
@@ -41,7 +41,7 @@ def level_k(P, j):
 
 
 def last_separate_batch(k, sm_count):
-    """the largest batch that still runs the separate kernels (keyswitch_core's rule)"""
+    """the largest batch that still runs the separate kernels (keyswitch_accumulate's rule)"""
     return (2 * sm_count) // (k * (k + 1))
 
 

@@ -54,7 +54,7 @@ def level_kr(P, j):
 
 
 def ks_batch(P, j, side):
-    """a batch on `side` ("below" / "at") of keyswitch_core's cluster rule k (k + 1) batch > 2 sm_count (k = 1: that of k = 2)"""
+    """a batch on `side` ("below" / "at") of keyswitch_accumulate's cluster rule k (k + 1) batch > 2 sm_count (k = 1: that of k = 2)"""
     return side_batch(max(level_kr(P, j)[0], 2), P.ctx.sm_count, side)
 
 

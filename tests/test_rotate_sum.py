@@ -38,7 +38,7 @@ def level_k(P, j):
 
 
 def cluster_batch(P, j, side):
-    """a batch just below ("below") or just above ("at") keyswitch_core's cluster rule k (k + 1) batch > 2 sm_count"""
+    """a batch just below ("below") or just above ("at") keyswitch_accumulate's cluster rule k (k + 1) batch > 2 sm_count"""
     k = max(level_k(P, j), 2)
     last = (2 * P.ctx.sm_count) // (k * (k + 1))
     return max(1, last) if side == "below" else last + 1
