@@ -240,6 +240,12 @@ void b200_trace_dump(void);
    queries it to size the grid of the persistent kernel; B200_E_INVALID when no such kernel exists.
    Meaningful once a context exists (context creation raises the kernels' shared-memory limit) */
 int b200_debug_ntt_ctas_per_sm(int logn, int forward, int threads);
+/* developer aid: device prime `prime_index` (key primes, then the auxiliary primes, then the plain modulus when batching) in
+   *prime (0: no such prime), and its FP64 transform's renorm masks (bit i: renormalise the inputs of pass i in execution
+   order).  schedule 0: the masks the context's transforms use; 1: those of the generic pass schedule; 2: those of the
+   statically scheduled kernels (n = 4096 ... 16384 only).  B200_E_INVALID for no such prime, a prime off the FP64 path or a
+   schedule the size does not have */
+int b200_debug_fp_masks(const b200_ctx *ctx, int prime_index, int schedule, uint64_t *prime, unsigned *fwd, unsigned *inv);
 
 #ifdef __cplusplus
 }

@@ -1235,6 +1235,14 @@ struct LevelFpHost
     int k = 0, nB = 0, nBsk = 0;
 };
 
+// renorm masks of one FP64 prime: [0] for the generic pass schedule, [1] for the statically scheduled kernels' (has_static)
+struct FpMasks
+{
+    unsigned fwd[2] = { 0, 0 }, inv[2] = { 0, 0 };
+    bool has_static = false;
+    int running = 0; // the schedule whose masks the transforms use
+};
+
 struct b200_ctx
 {
     std::vector<LevelFpHost> fp_levels; // indexed like `levels`; empty tables when the level is not on the FP64 path
@@ -1250,6 +1258,8 @@ struct b200_ctx
     NttPrimeFp *d_fp_primes = nullptr;
     bool fp_enabled = false;
     std::vector<bool> prime_fp;  // per device prime: takes the FP64 path
+    std::vector<FpMasks> fp_masks; // per device prime (FP64 path): renorm masks per schedule (b200_debug_fp_masks)
+    std::vector<u64> prime_value;  // per device prime
     int plain_prime_idx = -1;    // index of the plain modulus in the device prime tables (-1: no batching)
     PrimeDev *d_primes = nullptr;       // [all primes] key primes first
     std::vector<LevelDev> levels;       // device pointers inside
@@ -1363,11 +1373,15 @@ static int build_device(b200_ctx *ctx)
     UP(pd, &ctx->d_primes);
     {
         // FP64 fast path descriptors + magnitude bookkeeping (see ntt_fp_body.cuh).  All intermediates must stay
-        // below 2^51; a forward stage adds < p to the bound, an inverse stage doubles it.
+        // integers of magnitude <= 2^53; a forward stage adds a product bound, an inverse stage doubles it.
         const bool no_fp = std::getenv("B200_NO_FP64_NTT") != nullptr || ctx->ntt_split;
         ctx->fp_enabled = !no_fp;
         std::vector<NttPrimeFp> fp(allp.size());
         ctx->prime_fp.assign(allp.size(), false);
+        ctx->fp_masks.assign(allp.size(), FpMasks{});
+        ctx->prime_value.resize(allp.size());
+        for (size_t i = 0; i < allp.size(); i++)
+            ctx->prime_value[i] = allp[i]->mod.p;
         for (size_t i = 0; i < allp.size(); i++)
         {
             auto &P = *allp[i];
@@ -1414,68 +1428,21 @@ static int build_device(b200_ctx *ctx)
                 UP(i16, &d16);
                 fp[i].inv16 = d16;
             }
-            // Magnitude bookkeeping.  Every stored value must stay an exactly representable integer (|x| <= 2^53), and a
-            // modular product y*w - rint(fl(fl(y*w) * fl(1/p))) * p of an input |y| <= 2^53 has magnitude at most
-            // p * (1/2 + 3 * 2^-53 * |y|)  (three roundings of relative size 2^-53 in the quotient, one rint), computed
-            // exactly (ntt_fp_body.cuh).  Forward butterfly: X +- T.  Inverse butterfly: X + Y and (X - Y) * w.
-            const double LIMIT = 9007199254740992.0; // 2^53
-            auto prod_bound = [&](double y) { return p * (0.5 + 3.0 * y / LIMIT) + 1.0; };
-            const double RENORMED = 0.76 * p;       // |x - rint(x/p) p| after fp_renorm / fp_renorm_x
-            auto fwd_pass = [&](double b, int L, bool &ok) {
-                for (int s = 0; s < L; s++)
-                {
-                    b += prod_bound(b);
-                    ok = ok && b <= LIMIT;
-                }
-                return b;
-            };
-            auto inv_pass = [&](double b, int L, bool &ok) {
-                for (int s = 0; s < L; s++)
-                {
-                    ok = ok && 2.0 * b <= LIMIT;
-                    b = std::max(2.0 * b, prod_bound(2.0 * b));
-                }
-                return b;
-            };
-            // the pass schedule that will run: the statically scheduled kernel's where it is used, else the generic one
-            int sched_np = ctx->npass, sched_L[8];
-            for (int pi = 0; pi < ctx->npass; pi++)
-                sched_L[pi] = ctx->pass_L[pi];
+            // renorm masks (magnitude bookkeeping: ntt_fp_body.cuh fp_renorm_masks) for the generic pass schedule and, at the
+            // sizes that have one, for the statically scheduled kernels'; the transforms get those of the schedule that runs
+            FpMasks &m = ctx->fp_masks[i];
+            int sL[4];
+            const int snp = ntt_static_schedule(ctx->logn, sL);
+            if (!fp_renorm_masks(p, ctx->npass, ctx->pass_L, m.fwd[0], m.inv[0]) || (snp && !fp_renorm_masks(p, snp, sL, m.fwd[1], m.inv[1])))
+                return fail(B200_E_LOGIC, "internal: FP64 NTT bound analysis failed");
+            m.has_static = snp != 0;
 #ifndef B200_EMU_HEADER
-            if (ctx->logn >= 12 && ctx->logn <= 14 && !std::getenv("B200_NO_STATIC_NTT"))
-                sched_np = ntt_static_schedule(ctx->logn, sched_L);
+            m.running = m.has_static && !std::getenv("B200_NO_STATIC_NTT") ? 1 : 0;
+#else
+            m.running = 0; // the emulation runs the generic schedule at every size
 #endif
-            double B = p; // canonical (or Barrett-reduced) input
-            for (int pi = 0; pi < sched_np; pi++)
-            {
-                bool ok = true;
-                double nb = fwd_pass(B, sched_L[pi], ok);
-                if (!ok)
-                {
-                    fp[i].renorm_fwd |= 1u << pi;
-                    ok = true;
-                    nb = fwd_pass(RENORMED, sched_L[pi], ok);
-                    if (!ok)
-                        return fail(B200_E_LOGIC, "internal: FP64 NTT bound analysis failed (forward)");
-                }
-                B = nb;
-            }
-            B = p;
-            int step = 0;
-            for (int pi = sched_np - 1; pi >= 0; pi--, step++)
-            {
-                bool ok = true;
-                double nb = inv_pass(B, sched_L[pi], ok);
-                if (!ok)
-                {
-                    fp[i].renorm_inv |= 1u << step;
-                    ok = true;
-                    nb = inv_pass(RENORMED, sched_L[pi], ok);
-                    if (!ok)
-                        return fail(B200_E_LOGIC, "internal: FP64 NTT bound analysis failed (inverse)");
-                }
-                B = nb;
-            }
+            fp[i].renorm_fwd = m.fwd[m.running];
+            fp[i].renorm_inv = m.inv[m.running];
         }
         UP(fp, &ctx->d_fp_primes);
     }
@@ -2665,6 +2632,25 @@ int b200_debug_ntt_ctas_per_sm(int logn, int forward, int threads)
     (void)threads;
     return fail(B200_E_INVALID, "the emulation build has no FP64 NTT kernels");
 #endif
+}
+
+int b200_debug_fp_masks(const b200_ctx *ctx, int prime_index, int schedule, uint64_t *prime, unsigned *fwd, unsigned *inv)
+{
+    if (!ctx || !prime || !fwd || !inv)
+        return fail(B200_E_NULL, "null argument");
+    *prime = 0;
+    if (prime_index < 0 || prime_index >= (int)ctx->prime_fp.size())
+        return fail(B200_E_INVALID, "no such prime");
+    *prime = ctx->prime_value[prime_index];
+    if (!ctx->prime_fp[prime_index])
+        return fail(B200_E_INVALID, "not a prime of the FP64 path");
+    const FpMasks &m = ctx->fp_masks[prime_index];
+    if (schedule < 0 || schedule > 2 || (schedule == 2 && !m.has_static))
+        return fail(B200_E_INVALID, "no such schedule at this size");
+    const int s = schedule == 0 ? m.running : schedule - 1;
+    *fwd = m.fwd[s];
+    *inv = m.inv[s];
+    return 0;
 }
 
 void b200_trace_dump(void)

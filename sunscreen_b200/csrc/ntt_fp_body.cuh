@@ -1,4 +1,4 @@
-// ntt_fp_body.cuh — the FP64-pipe negacyclic NTT / INTT for primes below 2^47 (fast path for GPUs with a full-rate FP64 pipe).
+// ntt_fp_body.cuh — the FP64-pipe negacyclic NTT / INTT for primes up to 49 bits (fast path for GPUs with a full-rate FP64 pipe).
 //
 // Why: the 64-bit integer butterfly is bound by the wide integer multiply (IMAD.WIDE.U32 / IMAD.HI chains; tools/ubench.cu
 // measures the pipe rates), while H100 issues DFMA/DMUL/DADD at 64 lanes/clk/SM (its full-rate FP64 pipe).  A modular
@@ -48,6 +48,12 @@ __device__ __forceinline__ double b200_rint(double x)
 #define B200_MAGIC 6755399441055744.0   /* 1.5 * 2^52 */
 #define B200_TWO52 4503599627370496.0   /* 2^52 */
 
+// Test hook: every value a transform pass writes (its direction, its log2 sub-stride, the lazy value) before it is stored.
+// Empty in the product; tests/fp_exact records the largest magnitude per pass against the bookkeeping's bound.
+#ifndef B200_FP_AUDIT
+#define B200_FP_AUDIT(fwd, logs, x) ((void)0)
+#endif
+
 struct NttPrimeFp
 {
     double p, pinv;
@@ -65,7 +71,8 @@ B200_HD double fp_mulmod(double y, double w, double wp, double p)
     const double h = B200_DMUL(y, w);
     const double l = B200_DFMA(y, w, -h);
     // magic-number rounding (two FP64 slots): the element-wise BEHZ kernels that use this form issue almost nothing
-    // but modular products, and routing all their roundings through the 16-lane XU pipe was measured slower
+    // but modular products, and routing all their roundings through the 16-lane XU pipe was measured slower.  The
+    // magic-number rounding is exact only while |y*wp| < 2^51; the BEHZ kernels pass |y| < 2^49 and w < p
     const double q = B200_DADD(B200_DFMA(y, wp, B200_MAGIC), -B200_MAGIC);
     return B200_DADD(B200_DFMA(-q, p, h), l);
 }
@@ -87,7 +94,10 @@ B200_HD double fp_mulmod_term(int i, double y, double w, double wp, double p)
 {
     return (B200_BEHZ_XU_MIX && (i & 1)) ? fp_mulmod_x(y, w, wp, p) : fp_mulmod(y, w, wp, p);
 }
-// general product a*b mod p for |a|,|b| < 2^47 (no precomputed quotient): result in (-p, p)
+// general product a*b mod p (no precomputed quotient), exact for integer-valued |a| <= 2^53 and |b| < p < 2^49: the quotient
+// rint(fl(fl(a*b) * fl(1/p))) carries three roundings, so the result has magnitude <= p (1/2 + 3 |a| 2^-53) + 1
+// (fp_prod_bound; tests/test_fp_exact.py checks it at the rounding boundaries).  The transform's butterflies multiply lazy
+// values up to 2^53 by twiddles; the inner products multiply canonical values (result within p/2 + 1 + 3 p^2 2^-53).
 B200_HD double fp_mulmod2(double a, double b, double p, double pinv)
 {
     const double h = B200_DMUL(a, b);
@@ -95,6 +105,7 @@ B200_HD double fp_mulmod2(double a, double b, double p, double pinv)
     const double q = B200_RINT(B200_DMUL(h, pinv));
     return B200_DADD(B200_DFMA(-q, p, h), l);
 }
+// x - rint(x/p) p for |x| <= 2^53: magnitude <= fp_renormed_bound(p)
 B200_HD double fp_renorm(double x, double p, double pinv)
 {
     const double q = B200_DADD(B200_DFMA(x, pinv, B200_MAGIC), -B200_MAGIC);
@@ -113,7 +124,7 @@ B200_HD u64 fp_to_canonical(double x, double p, double pinv)
     double r = XU ? fp_renorm_x(x, p, pinv) : fp_renorm(x, p, pinv); // |r| <= 0.76 p
     r = r < 0.0 ? B200_DADD(r, p) : r;
 #if defined(__CUDA_ARCH__)
-    return (u64)__double_as_longlong(r + B200_TWO52) & 0x000FFFFFFFFFFFFFULL; // exact: 0 <= r < 2^47
+    return (u64)__double_as_longlong(r + B200_TWO52) & 0x000FFFFFFFFFFFFFULL; // exact: 0 <= r < p < 2^49
 #else
     return (u64)(long long)r;
 #endif
@@ -324,6 +335,7 @@ B200_HD void ntt_fp_group(double *sm, const u64 *__restrict__ gsrc, u64 *__restr
 #pragma unroll
     for (int j = 0; j < R; j++)
     {
+        B200_FP_AUDIT(FWD, logs, x[j]);
         if (DST_GLOBAL)
             gdst[base + (j << logs)] = fp_to_canonical<true>(x[j], p, P.pinv);
         else
@@ -409,17 +421,78 @@ B200_HD void ntt_fp_block_body(const NttJob &job, const NttPrimeFp &P, const Ntt
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Statically scheduled variant (device fast path): compile-time pass schedule and thread count, group loops
-// fully unrolled so that all global loads of the first pass are issued before the first butterfly.
-// Same group routine as above (which the CPU emulation tests cover); only the control flow is specialised.
+// Magnitude bookkeeping (host: b200_bfv.cu build_device sets every prime's renorm masks with it).  Every stored value
+// must stay an exactly representable integer (|x| <= 2^53).  A modular product y*w - rint(fl(fl(y*w) * fl(1/p))) * p of an
+// input |y| <= 2^53 and a twiddle w < p has magnitude at most fp_prod_bound(p, |y|) (three roundings of relative size 2^-53
+// in the quotient, one rint), computed exactly (fp_mulmod2).  Forward butterfly: X +- T.  Inverse butterfly: X + Y and
+// (X - Y) * w.  Renormalised inputs (fp_renorm_x) have magnitude at most fp_renormed_bound(p).
 // ---------------------------------------------------------------------------------------------------------
-#if defined(__CUDACC__)
+#define B200_FP_LIMIT 9007199254740992.0 /* 2^53 */
+inline double fp_prod_bound(double p, double y) { return p * (0.5 + 3.0 * y / B200_FP_LIMIT) + 1.0; }
+inline double fp_renormed_bound(double p) { return 0.76 * p; }
+// bit i of fwd / inv: renormalise the inputs of pass i (execution order) of the forward schedule L[0..np) / its mirror image.
+// Returns false when a pass could exceed 2^53 even on renormalised inputs.
+inline bool fp_renorm_masks(double p, int np, const int *L, unsigned &fwd, unsigned &inv)
+{
+    auto fwd_pass = [&](double b, int stages, bool &ok) {
+        for (int s = 0; s < stages; s++)
+        {
+            b += fp_prod_bound(p, b);
+            ok = ok && b <= B200_FP_LIMIT;
+        }
+        return b;
+    };
+    auto inv_pass = [&](double b, int stages, bool &ok) {
+        for (int s = 0; s < stages; s++)
+        {
+            ok = ok && 2.0 * b <= B200_FP_LIMIT;
+            const double pb = fp_prod_bound(p, 2.0 * b);
+            b = 2.0 * b > pb ? 2.0 * b : pb;
+        }
+        return b;
+    };
+    fwd = inv = 0;
+    double B = p; // canonical (or Barrett-reduced) input
+    for (int pi = 0; pi < np; pi++)
+    {
+        bool ok = true;
+        double nb = fwd_pass(B, L[pi], ok);
+        if (!ok)
+        {
+            fwd |= 1u << pi;
+            ok = true;
+            nb = fwd_pass(fp_renormed_bound(p), L[pi], ok);
+            if (!ok)
+                return false;
+        }
+        B = nb;
+    }
+    B = p;
+    int step = 0;
+    for (int pi = np - 1; pi >= 0; pi--, step++)
+    {
+        bool ok = true;
+        double nb = inv_pass(B, L[pi], ok);
+        if (!ok)
+        {
+            inv |= 1u << step;
+            ok = true;
+            nb = inv_pass(fp_renormed_bound(p), L[pi], ok);
+            if (!ok)
+                return false;
+        }
+        B = nb;
+    }
+    return true;
+}
+
+// The statically scheduled kernels' pass schedules (below), also for the host's magnitude bookkeeping: renorm masks are
+// per pass of the schedule that runs.
 template <int LOGN> struct NttSched;
 template <> struct NttSched<12> { static constexpr int NP = 3; static constexpr int L0 = 4, L1 = 4, L2 = 4, L3 = 0; };
 template <> struct NttSched<13> { static constexpr int NP = 4; static constexpr int L0 = 3, L1 = 3, L2 = 3, L3 = 4; };
 template <> struct NttSched<14> { static constexpr int NP = 4; static constexpr int L0 = 3, L1 = 3, L2 = 4, L3 = 4; };
 
-// the same schedules for the host's magnitude bookkeeping (renorm masks are per pass of the schedule that runs)
 inline int ntt_static_schedule(int logn, int *L)
 {
     auto fill = [&](int np, int a, int b, int c_, int d) { L[0] = a; L[1] = b; L[2] = c_; L[3] = d; return np; };
@@ -431,6 +504,13 @@ inline int ntt_static_schedule(int logn, int *L)
         return fill(NttSched<14>::NP, NttSched<14>::L0, NttSched<14>::L1, NttSched<14>::L2, NttSched<14>::L3);
     return 0;
 }
+
+// ---------------------------------------------------------------------------------------------------------
+// Statically scheduled variant (device fast path): compile-time pass schedule and thread count, group loops
+// fully unrolled so that all global loads of the first pass are issued before the first butterfly.
+// Same group routine as above (which the CPU emulation tests cover); only the control flow is specialised.
+// ---------------------------------------------------------------------------------------------------------
+#if defined(__CUDACC__)
 template <int LOGN, int PI> struct NttSchedL
 {
     static constexpr int value = PI == 0 ? NttSched<LOGN>::L0 : PI == 1 ? NttSched<LOGN>::L1 : PI == 2 ? NttSched<LOGN>::L2 : NttSched<LOGN>::L3;
