@@ -1897,6 +1897,13 @@ static int check_level(b200_ctx *ctx, int level)
     return 0;
 }
 
+// whether the byte ranges [x, x + x_bytes) and [y, y + y_bytes) share a byte
+static bool overlaps(const void *x, uint64_t x_bytes, const void *y, uint64_t y_bytes)
+{
+    const uintptr_t a = (uintptr_t)x, b = (uintptr_t)y;
+    return a < b + y_bytes && b < a + x_bytes;
+}
+
 // slots over a dense [items][slots][n] slab with per-slot prime
 static int dense_job(b200_ctx *ctx, const std::string &key, const std::vector<int> &prime, JobDesc *jd)
 {
@@ -1913,6 +1920,12 @@ static std::vector<int> row_primes(b200_ctx *ctx, int level, bool with_bsk)
     if (with_bsk)
         r.insert(r.end(), Lh.bsk_idx.begin(), Lh.bsk_idx.end());
     return r;
+}
+
+// the level's k residues over a dense [items][k][n] slab
+static int slab_job(b200_ctx *ctx, int level, JobDesc *jd)
+{
+    return dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), jd);
 }
 
 // ---- multiply core: writes polys [0,split) to dst0 and [split,Dn) to dst1 ----
@@ -2860,7 +2873,7 @@ static int ntt_slab(b200_ctx *ctx, int level, u64 *data, uint64_t items, void *s
     if (!data)
         return fail(B200_E_NULL, "null data");
     JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+    if ((rc = slab_job(ctx, level, &jd)))
         return rc;
     const long long stride = (long long)ctx->levels[level].k * (long long)ctx->n;
     if (fwd)
@@ -3166,13 +3179,9 @@ int b200_multiply_relin_sum(b200_ctx *ctx, int level, const uint64_t *a, const u
     const LevelDev &L = ctx->levels[level];
     const int k = L.k, R = k + L.nBsk;
     const size_t w = (size_t)2 * k * n; // words of one ciphertext
-    {
-        const uintptr_t o0 = (uintptr_t)out2, o1 = o0 + rows * w * sizeof(u64);
-        const uintptr_t span = rows * m * w * sizeof(u64);
-        for (const uint64_t *x : { a, b })
-            if ((uintptr_t)x < o1 && o0 < (uintptr_t)x + span)
-                return fail(B200_E_INVALID, "multiply_relin_sum: out overlaps an operand");
-    }
+    for (const uint64_t *x : { a, b })
+        if (overlaps(x, rows * m * w * sizeof(u64), out2, rows * w * sizeof(u64)))
+            return fail(B200_E_INVALID, "multiply_relin_sum: out overlaps an operand");
     CU_TRY(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     // scratch of one term at its peak: c2 with D (or c0 / c1) held, plus the larger of the multiply's ext + D and the key
@@ -3312,13 +3321,9 @@ int b200_apply_galois_add(b200_ctx *ctx, int level, const uint64_t *in2, uint32_
     if (!(galois_elt & 1) || galois_elt >= 2 * ctx->n)
         return fail(B200_E_INVALID, "Galois element is not valid");
     const size_t bytes = (size_t)batch * 2 * ctx->levels[level].k * ctx->n * sizeof(u64);
-    auto overlap = [bytes](const void *a, const void *b) {
-        const char *x = (const char *)a, *y = (const char *)b;
-        return x < y + bytes && y < x + bytes;
-    };
-    if (batch && overlap(in2, out2))
+    if (batch && overlaps(in2, bytes, out2, bytes))
         return fail(B200_E_INVALID, "apply_galois_add: out overlaps in");
-    if (batch && addend2 && addend2 != out2 && overlap(addend2, out2))
+    if (batch && addend2 && addend2 != out2 && overlaps(addend2, bytes, out2, bytes))
         return fail(B200_E_INVALID, "apply_galois_add: addend overlaps out without being out");
     if (batch == 0)
         return 0;
@@ -3360,12 +3365,8 @@ int b200_apply_galois_many(b200_ctx *ctx, int level, const uint64_t *in2, const 
             return fail(B200_E_NULL, "null key");
         sources = std::max(sources, (src_idx ? src_idx[i] : i) + 1);
     }
-    {
-        const uintptr_t x0 = (uintptr_t)in2, x1 = x0 + (uintptr_t)(sources * w * sizeof(u64));
-        const uintptr_t o0 = (uintptr_t)out2, o1 = o0 + (uintptr_t)(batch * w * sizeof(u64));
-        if (x0 < o1 && o0 < x1)
-            return fail(B200_E_INVALID, "apply_galois_many: out overlaps in");
-    }
+    if (overlaps(in2, sources * w * sizeof(u64), out2, batch * w * sizeof(u64)))
+        return fail(B200_E_INVALID, "apply_galois_many: out overlaps in");
     CU_TRY(cudaSetDevice(ctx->device));
     std::vector<B200GalItem> tab(batch);
     for (uint64_t i = 0; i < batch; i++)
@@ -3400,7 +3401,7 @@ static int plain_lift_ntt(b200_ctx *ctx, int level, const u64 *plain, uint64_t p
         ctx->launches++;
     }
     JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+    if ((rc = slab_job(ctx, level, &jd)))
         return rc;
     return launch_ntt<true>(ctx, jd, out, (long long)k * n, out, (long long)k * n, (long long)pb, 0, s);
 }
@@ -3428,7 +3429,7 @@ int b200_multiply_plain(b200_ctx *ctx, int level, const uint64_t *a, int size, c
     if ((rc = plain_lift_ntt(ctx, level, (const u64 *)plain, pb, pl, true, scr, s)))
         return rc;
     JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+    if ((rc = slab_job(ctx, level, &jd)))
         return rc;
     // ct polys: forward (out of place), dyadic, inverse
     if ((rc = launch_ntt<true>(ctx, jd, (const u64 *)a, (long long)k * n, (u64 *)out, (long long)k * n, (long long)batch * size, 0,
@@ -3467,6 +3468,16 @@ int b200_plain_to_ntt(b200_ctx *ctx, int level, const uint64_t *plain, uint64_t 
     return 0;
 }
 
+// the plaintext MACs' products summed between two reductions: r + lazy (q - 1)^2 < 2^128 for a remainder r < q of the
+// previous chunk, for every prime q of the level
+static int mac_lazy_terms(b200_ctx *ctx, int level)
+{
+    int bits = 0;
+    for (int qi : ctx->host->levels[level].q_idx)
+        bits = std::max(bits, 64 - __builtin_clzll(ctx->host->primes[qi].mod.p));
+    return bits <= 60 ? 256 : 1 << (128 - 2 * bits);
+}
+
 // Sums of multiply_plain products: out[i] = INTT(sum_j NTT(cts[j]) (*) plain_ntt[i][j]).  The inverse NTT is linear mod q and
 // every hand-off is canonical, so the words equal those of multiply_plain(cts[0], p_i0) + ... + multiply_plain(cts[m-1], ...)
 // while each ciphertext is transformed once and each output once.
@@ -3486,12 +3497,8 @@ int b200_multiply_plain_sum(b200_ctx *ctx, int level, const uint64_t *cts, int s
     const LevelHost &Lh = ctx->host->levels[level];
     const int k = Lh.k;
     const long long kn = (long long)k * n;
-    {
-        const uintptr_t x0 = (uintptr_t)cts, x1 = x0 + (uintptr_t)(m * size * kn * sizeof(u64));
-        const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (uintptr_t)(R * size * kn * sizeof(u64));
-        if (x0 < o1 && o0 < x1)
-            return fail(B200_E_INVALID, "out must not overlap cts");
-    }
+    if (overlaps(cts, m * size * kn * sizeof(u64), out, R * size * kn * sizeof(u64)))
+        return fail(B200_E_INVALID, "out must not overlap cts");
     CU_TRY(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
@@ -3499,18 +3506,11 @@ int b200_multiply_plain_sum(b200_ctx *ctx, int level, const uint64_t *cts, int s
     if ((rc = scr.get((size_t)m * size * kn, &X)))
         return rc;
     JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+    if ((rc = slab_job(ctx, level, &jd)))
         return rc;
     if ((rc = launch_ntt<true>(ctx, jd, (const u64 *)cts, kn, X, kn, (long long)m * size, 0, s)))
         return rc;
-    // terms between two reductions: r + lazy (q - 1)^2 < 2^128 for a remainder r < q of the previous chunk
-    int bits = 0;
-    for (int r = 0; r < k; r++)
-    {
-        const u64 q = ctx->host->primes[Lh.q_idx[r]].mod.p;
-        bits = std::max(bits, 64 - __builtin_clzll(q));
-    }
-    const int lazy = bits <= 60 ? 256 : 1 << (128 - 2 * bits);
+    const int lazy = mac_lazy_terms(ctx, level);
     const dim3 grid((unsigned)((R + MAC_ROWS - 1) / MAC_ROWS), blocks_for(kn / 2, MAC_NT));
     for (int c0 = 0; c0 < size; c0 += 3)
     {
@@ -3581,12 +3581,8 @@ int b200_linear_transform(b200_ctx *ctx, int level, const uint64_t *cts, uint64_
     const LevelHost &Lh = ctx->host->levels[level];
     const int k = Lh.k;
     const long long kn = (long long)k * n, w = 2 * kn;
-    {
-        const uintptr_t x0 = (uintptr_t)cts, x1 = x0 + (uintptr_t)(V * w * sizeof(u64));
-        const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (uintptr_t)(V * w * sizeof(u64));
-        if (V && out != cts && x0 < o1 && o0 < x1)
-            return fail(B200_E_INVALID, "out must be cts or not overlap it");
-    }
+    if (V && out != cts && overlaps(cts, V * w * sizeof(u64), out, V * w * sizeof(u64)))
+        return fail(B200_E_INVALID, "out must be cts or not overlap it");
     if (V == 0)
         return 0;
     CU_TRY(cudaSetDevice(ctx->device));
@@ -3599,12 +3595,9 @@ int b200_linear_transform(b200_ctx *ctx, int level, const uint64_t *cts, uint64_
         budget = std::max(1LL, atoll(e));
     const long long chunk = std::max(1LL, budget / (per * (long long)sizeof(u64)));
     JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+    if ((rc = slab_job(ctx, level, &jd)))
         return rc;
-    int bits = 0; // terms between two reductions of the MAC, as in b200_multiply_plain_sum
-    for (int r = 0; r < k; r++)
-        bits = std::max(bits, 64 - __builtin_clzll(ctx->host->primes[Lh.q_idx[r]].mod.p));
-    const int lazy = bits <= 60 ? 256 : 1 << (128 - 2 * bits);
+    const int lazy = mac_lazy_terms(ctx, level);
     std::vector<unsigned char> mask;
     if (present)
         mask.assign(present, present + (long long)G * b);
@@ -3758,29 +3751,30 @@ int b200_mod_switch_to_next(b200_ctx *ctx, int level, const uint64_t *a, int siz
     return 0;
 }
 
-int b200_decrypt(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, uint64_t *plain_out,
-                 uint64_t batch, void *stream)
+// the argument checks of the secret-key operations, in the order they are reported
+static int check_sk_args(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, const void *out)
 {
     int rc = check_level(ctx, level);
     if (rc)
         return rc;
-    if (!ct || !sk_powers_ntt || !plain_out)
+    if (!ct || !sk_powers_ntt || !out)
         return fail(B200_E_NULL, "null pointer");
     if (size < 2)
         return fail(B200_E_INVALID, "ciphertext size must be >= 2");
-    if (batch == 0)
-        return 0;
-    CU_TRY(cudaSetDevice(ctx->device));
+    return 0;
+}
+
+// ---- secret-key phase, all but c0: acc [batch][k][n] (coefficient form, canonical) = INTT(sum_{j>=1} NTT(c_j) * s^j) of the
+// ciphertexts ct [batch][size][k][n].  Each operation then adds c0 in its own last kernel. ----
+static int sk_phase(b200_ctx *ctx, int level, const u64 *ct, int size, const u64 *sk_powers_ntt, u64 *acc, long long batch,
+                    Scratch &scr, cudaStream_t s)
+{
     const long long n = (long long)ctx->n;
-    const LevelDev &L = ctx->levels[level];
     const LevelHost &Lh = ctx->host->levels[level];
-    const int k = L.k, terms = size - 1;
-    cudaStream_t s = (cudaStream_t)stream;
-    Scratch scr(ctx, s);
-    u64 *X = nullptr, *acc = nullptr;
+    const int k = ctx->levels[level].k, terms = size - 1;
+    u64 *X = nullptr;
+    int rc;
     if ((rc = scr.get((size_t)batch * terms * k * n, &X)))
-        return rc;
-    if ((rc = scr.get((size_t)batch * k * n, &acc)))
         return rc;
     {
         std::vector<int> prime;
@@ -3795,20 +3789,39 @@ int b200_decrypt(b200_ctx *ctx, int level, const uint64_t *ct, int size, const u
         JobDesc jd;
         if ((rc = get_job(ctx, "dec:" + std::to_string(level) + ":" + std::to_string(size), prime, so, dof, &jd)))
             return rc;
-        if ((rc = launch_ntt<true>(ctx, jd, (const u64 *)ct, (long long)size * k * n, X, (long long)terms * k * n,
-                                   (long long)batch, 0, s)))
+        if ((rc = launch_ntt<true>(ctx, jd, ct, (long long)size * k * n, X, (long long)terms * k * n, batch, 0, s)))
             return rc;
     }
     {
-        const long long total = (long long)batch * k * n;
-        B200_LAUNCH(dot_sk_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, terms, X, (const u64 *)sk_powers_ntt, acc,
-                                                           ctx->logn, total);
+        const long long total = batch * k * n;
+        B200_LAUNCH(dot_sk_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, terms, X, sk_powers_ntt, acc, ctx->logn,
+                    total);
         ctx->launches++;
     }
     JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
+    if ((rc = slab_job(ctx, level, &jd)))
         return rc;
-    if ((rc = launch_ntt<false>(ctx, jd, acc, (long long)k * n, acc, (long long)k * n, (long long)batch, 0, s)))
+    return launch_ntt<false>(ctx, jd, acc, (long long)k * n, acc, (long long)k * n, batch, 0, s);
+}
+
+int b200_decrypt(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, uint64_t *plain_out,
+                 uint64_t batch, void *stream)
+{
+    int rc = check_sk_args(ctx, level, ct, size, sk_powers_ntt, plain_out);
+    if (rc)
+        return rc;
+    if (batch == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    const long long n = (long long)ctx->n;
+    const LevelDev &L = ctx->levels[level];
+    const int k = L.k;
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    u64 *acc = nullptr;
+    if ((rc = scr.get((size_t)batch * k * n, &acc)))
+        return rc;
+    if ((rc = sk_phase(ctx, level, (const u64 *)ct, size, (const u64 *)sk_powers_ntt, acc, (long long)batch, scr, s)))
         return rc;
     {
         const long long total = (long long)batch * n;
@@ -3824,53 +3837,18 @@ int b200_decrypt(b200_ctx *ctx, int level, const uint64_t *ct, int size, const u
 int b200_ct_sk_phase(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, uint64_t *phase_out,
                      uint64_t batch, void *stream)
 {
-    int rc = check_level(ctx, level);
+    int rc = check_sk_args(ctx, level, ct, size, sk_powers_ntt, phase_out);
     if (rc)
         return rc;
-    if (!ct || !sk_powers_ntt || !phase_out)
-        return fail(B200_E_NULL, "null pointer");
-    if (size < 2)
-        return fail(B200_E_INVALID, "ciphertext size must be >= 2");
     if (batch == 0)
         return 0;
     CU_TRY(cudaSetDevice(ctx->device));
     const long long n = (long long)ctx->n;
-    const LevelDev &L = ctx->levels[level];
-    const LevelHost &Lh = ctx->host->levels[level];
-    const int k = L.k, terms = size - 1;
+    const int k = ctx->levels[level].k;
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
-    u64 *X = nullptr;
     u64 *acc = (u64 *)phase_out;
-    if ((rc = scr.get((size_t)batch * terms * k * n, &X)))
-        return rc;
-    {
-        std::vector<int> prime;
-        std::vector<long long> so, dof;
-        for (int j = 0; j < terms; j++)
-            for (int r = 0; r < k; r++)
-            {
-                prime.push_back(Lh.q_idx[r]);
-                so.push_back(((long long)(j + 1) * k + r) * n);
-                dof.push_back(((long long)j * k + r) * n);
-            }
-        JobDesc jd;
-        if ((rc = get_job(ctx, "dec:" + std::to_string(level) + ":" + std::to_string(size), prime, so, dof, &jd)))
-            return rc;
-        if ((rc = launch_ntt<true>(ctx, jd, (const u64 *)ct, (long long)size * k * n, X, (long long)terms * k * n,
-                                   (long long)batch, 0, s)))
-            return rc;
-    }
-    {
-        const long long total = (long long)batch * k * n;
-        B200_LAUNCH(dot_sk_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, terms, X, (const u64 *)sk_powers_ntt, acc,
-                    ctx->logn, total);
-        ctx->launches++;
-    }
-    JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
-        return rc;
-    if ((rc = launch_ntt<false>(ctx, jd, acc, (long long)k * n, acc, (long long)k * n, (long long)batch, 0, s)))
+    if ((rc = sk_phase(ctx, level, (const u64 *)ct, size, (const u64 *)sk_powers_ntt, acc, (long long)batch, scr, s)))
         return rc;
     {
         const long long total = (long long)batch * n;
@@ -3888,18 +3866,13 @@ int b200_ct_sk_phase(b200_ctx *ctx, int level, const uint64_t *ct, int size, con
 int b200_noise_norm(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, uint64_t *norm_out,
                     int words, uint64_t batch, void *stream)
 {
-    int rc = check_level(ctx, level);
+    int rc = check_sk_args(ctx, level, ct, size, sk_powers_ntt, norm_out);
     if (rc)
         return rc;
-    if (!ct || !sk_powers_ntt || !norm_out)
-        return fail(B200_E_NULL, "null pointer");
-    if (size < 2)
-        return fail(B200_E_INVALID, "ciphertext size must be >= 2");
     CU_TRY(cudaSetDevice(ctx->device));
     const long long n = (long long)ctx->n;
-    const LevelDev &L = ctx->levels[level];
     const LevelHost &Lh = ctx->host->levels[level];
-    const int k = L.k, terms = size - 1;
+    const int k = ctx->levels[level].k;
     u64 *consts = nullptr;
     int W = 0;
     {
@@ -3960,42 +3933,14 @@ int b200_noise_norm(b200_ctx *ctx, int level, const uint64_t *ct, int size, cons
         return 0;
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
-    u64 *X = nullptr, *acc = nullptr, *bm = nullptr;
+    u64 *acc = nullptr, *bm = nullptr;
     const int NT = 128, CHUNK = 128, WW = W + 1;
     const int blocks = (int)((n + CHUNK - 1) / CHUNK);
-    if ((rc = scr.get((size_t)batch * terms * k * n, &X)))
-        return rc;
     if ((rc = scr.get((size_t)batch * k * n, &acc)))
         return rc;
     if ((rc = scr.get((size_t)batch * blocks * WW, &bm)))
         return rc;
-    {
-        std::vector<int> prime;
-        std::vector<long long> so, dof;
-        for (int j = 0; j < terms; j++)
-            for (int r = 0; r < k; r++)
-            {
-                prime.push_back(Lh.q_idx[r]);
-                so.push_back(((long long)(j + 1) * k + r) * n);
-                dof.push_back(((long long)j * k + r) * n);
-            }
-        JobDesc jd;
-        if ((rc = get_job(ctx, "dec:" + std::to_string(level) + ":" + std::to_string(size), prime, so, dof, &jd)))
-            return rc;
-        if ((rc = launch_ntt<true>(ctx, jd, (const u64 *)ct, (long long)size * k * n, X, (long long)terms * k * n,
-                                   (long long)batch, 0, s)))
-            return rc;
-    }
-    {
-        const long long total = (long long)batch * k * n;
-        B200_LAUNCH(dot_sk_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, terms, X, (const u64 *)sk_powers_ntt, acc,
-                    ctx->logn, total);
-        ctx->launches++;
-    }
-    JobDesc jd;
-    if ((rc = dense_job(ctx, "slab:" + std::to_string(level), row_primes(ctx, level, false), &jd)))
-        return rc;
-    if ((rc = launch_ntt<false>(ctx, jd, acc, (long long)k * n, acc, (long long)k * n, (long long)batch, 0, s)))
+    if ((rc = sk_phase(ctx, level, (const u64 *)ct, size, (const u64 *)sk_powers_ntt, acc, (long long)batch, scr, s)))
         return rc;
     {
         dim3 grid((unsigned)blocks, (unsigned)batch);

@@ -172,6 +172,8 @@ def test_layer1_argument_checks(emu_lib):
         ("mod_switch at the last level", L.b200_mod_switch_to_next, (h, ci(ctx.levels - 1), p, ci(2), p, u64(1), None), E_INVALID),
         ("decrypt null", L.b200_decrypt, (h, ci(lv), p, ci(2), None, p, u64(1), None), E_NULL),
         ("decrypt size 1", L.b200_decrypt, (h, ci(lv), p, ci(1), p, p, u64(1), None), E_INVALID),
+        ("ct_sk_phase size 1", L.b200_ct_sk_phase, (h, ci(lv), p, ci(1), p, p, u64(1), None), E_INVALID),
+        ("noise_norm null key", L.b200_noise_norm, (h, ci(lv), p, ci(2), None, p, ci(k + 1), u64(1), None), E_NULL),
         ("multiply_relin_host null", L.b200_multiply_relin_host, (h, ci(lv), None, p, p, p, u64(1)), E_NULL),
         ("level_info bad level", L.b200_ctx_level_info, (h, ci(50), p), E_INVALID),
         ("galois_elt_from_step too large", L.b200_galois_elt_from_step, (h, ci(n), p), E_INVALID),
