@@ -38,6 +38,18 @@ int data_level(Context_ *c, const Ciphertext_ &ct, const char *what)
         throw InvalidArg(what);
     return lv;
 }
+// the level of a batch's items, which must be valid size-2 ciphertexts, not in NTT form, all at one level
+int batch_level(Context_ *c, uint64_t count, void **cts)
+{
+    const int lv = data_level(c, *(Ciphertext_ *)cts[0], "encrypted is not valid for encryption parameters");
+    for (uint64_t i = 0; i < count; i++)
+    {
+        auto &a = *(Ciphertext_ *)cts[i];
+        if (data_level(c, a, "encrypted is not valid for encryption parameters") != lv || a.size != 2 || a.is_ntt_form)
+            throw InvalidArg("batch items must be size-2 ciphertexts at the same level");
+    }
+    return lv;
+}
 
 void transparent_guard(Context_ *c, int level, Ciphertext_ &dst)
 {
@@ -178,24 +190,40 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
         const u64 in_polys = r0.kind == 1 ? 3 : 2, out_polys = r0.kind == 0 ? 3 : 2;
         const u64 win = in_polys * k * n, wout = out_polys * k * n;
         const size_t operands = r0.kind == 0 ? 2 : 1;
+        // An upload may reallocate an operand's device buffer, whose size the alias test below reads: every operand's device
+        // copy is made current first.
+        for (auto *r : batch)
+        {
+            r->a->dev_ptr(c);
+            if (operands == 2)
+                r->b->dev_ptr(c);
+        }
+        // the gather must read an aliased operand before prepare_output may release its buffer: when a destination is also
+        // an operand of DIFFERENT shape, fall back to the order gather -> prepare (no graph for that rare batch)
+        bool reshaped_alias = false;
+        for (size_t i = 0; i < N && !reshaped_alias; i++)
+            for (size_t j = 0; j < N; j++)
+                if ((batch[i]->dst == batch[j]->a || batch[i]->dst == batch[j]->b) && batch[i]->dst->dev_words < wout)
+                    reshaped_alias = true;
+        const bool graphs = c->use_graphs && !reshaped_alias;
         // With graphs the batch is padded to a power of two (the pad items repeat item 0 and write to a scratch destination):
         // far fewer distinct graph shapes per lane, at the price of a few wasted items in a latency-bound launch sequence.
-        size_t NP = N;
-        if (c->use_graphs)
-            for (NP = 1; NP < N; NP <<= 1)
+        size_t count = N;
+        if (graphs)
+            for (count = 1; count < N; count <<= 1)
                 ;
         // Everything that varies from call to call goes through the lane's pinned tables (addresses fixed for the lane's
         // lifetime, read directly by the kernels): operand pointers, destination pointers, transparent-result flags.
         u64 **tab = lane.hptrs, **dtab = tab + 2 * Context_::COMBINE_MAX;
         uint32_t *flags = lane.hflag;
-        for (size_t i = 0; i < NP; i++)
+        for (size_t i = 0; i < count; i++)
         {
             const size_t src = i < N ? i : 0;
             tab[i] = const_cast<u64 *>(batch[src]->a->dev_ptr(c));
             if (operands == 2)
-                tab[NP + i] = const_cast<u64 *>(batch[src]->b->dev_ptr(c));
+                tab[count + i] = const_cast<u64 *>(batch[src]->b->dev_ptr(c));
         }
-        if (NP > N && lane.pad_words < wout)
+        if (count > N && lane.pad_words < wout)
         {
             if (lane.pad_out)
                 b200_free_async(c->dev, lane.pad_out, cur_stream());
@@ -208,70 +236,59 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
         // An operand that IS a destination keeps its buffer (prepare_output reuses it when the capacity suffices); when the
         // shapes differ the old buffer is released in stream order, after the gather that reads it.
         const u64 *key = r0.kind == 0 ? nullptr : r0.keys->flat_dev(c, r0.kind == 1 ? 0 : r0.key_index, (int)k);
-        auto enqueue = [&]() -> int { // never throws: it also runs inside a stream capture, which must always be ended
-            void *pin = nullptr, *pout = nullptr;
-            int rc = b200_malloc_async(c->dev, operands * NP * win * sizeof(u64), &pin, cur_stream());
+        auto prepare = [&] {
+            for (size_t i = 0; i < count; i++)
+                dtab[i] = i < N ? batch[i]->dst->prepare_output(c, c->ids[lv], out_polys, k) : lane.pad_out;
+        };
+        // The launch sequence of the batch: allocate -> gather -> layer-1 call -> `place()` -> scatter -> transparent flags.
+        // Its two slabs are freed in stream order on every exit.  Only `place` may throw: inside a stream capture, which must
+        // always be ended, it does nothing.
+        auto sequence = [&](auto place) -> int {
+            struct Slabs
+            {
+                Context_ *c;
+                void *in = nullptr, *out = nullptr;
+                ~Slabs()
+                {
+                    if (in)
+                        b200_free_async(c->dev, in, cur_stream());
+                    if (out)
+                        b200_free_async(c->dev, out, cur_stream());
+                }
+            } s{ c };
+            int rc = b200_malloc_async(c->dev, operands * count * win * sizeof(u64), &s.in, cur_stream());
             if (!rc)
-                rc = b200_malloc_async(c->dev, NP * wout * sizeof(u64), &pout, cur_stream());
-            u64 *in = (u64 *)pin, *out = (u64 *)pout;
+                rc = b200_malloc_async(c->dev, count * wout * sizeof(u64), &s.out, cur_stream());
+            if (rc)
+                return rc;
+            u64 *in = (u64 *)s.in, *out = (u64 *)s.out;
+            rc = b200_gather_scatter_table(c->dev, tab, operands * count, in, win, 1, cur_stream());
             if (!rc)
-                rc = b200_gather_scatter_table(c->dev, tab, operands * NP, in, win, 1, cur_stream());
+                rc = r0.kind == 0   ? b200_multiply(c->dev, lv, in, 2, in + count * win, 2, out, count, cur_stream())
+                     : r0.kind == 1 ? b200_relinearize(c->dev, lv, in, key, out, count, cur_stream())
+                                    : b200_apply_galois(c->dev, lv, in, r0.elt, key, out, count, cur_stream());
+            place();
             if (!rc)
-                rc = r0.kind == 0   ? b200_multiply(c->dev, lv, in, 2, in + NP * win, 2, out, NP, cur_stream())
-                     : r0.kind == 1 ? b200_relinearize(c->dev, lv, in, key, out, NP, cur_stream())
-                                    : b200_apply_galois(c->dev, lv, in, r0.elt, key, out, NP, cur_stream());
-            if (!rc)
-                rc = b200_gather_scatter_table(c->dev, dtab, NP, out, wout, 0, cur_stream());
+                rc = b200_gather_scatter_table(c->dev, dtab, count, out, wout, 0, cur_stream());
             if (!rc && c->check_transparent)
-                rc = b200_any_nonzero(c->dev, lv, out, (int)out_polys, flags, NP, cur_stream());
-            if (pin)
-                b200_free_async(c->dev, pin, cur_stream());
-            if (pout)
-                b200_free_async(c->dev, pout, cur_stream());
+                rc = b200_any_nonzero(c->dev, lv, out, (int)out_polys, flags, count, cur_stream());
             return rc;
         };
-        // the gather must read an aliased operand before prepare_output may release its buffer: when a destination is also
-        // an operand of DIFFERENT shape, fall back to the order gather -> prepare (no graph for that rare batch)
-        bool reshaped_alias = false;
-        for (size_t i = 0; i < N && !reshaped_alias; i++)
-            for (size_t j = 0; j < N; j++)
-                if ((batch[i]->dst == batch[j]->a || batch[i]->dst == batch[j]->b) && batch[i]->dst->dev_words < wout)
-                    reshaped_alias = true;
+        auto enqueue = [&] { return sequence([] {}); };
         if (c->check_transparent)
-            for (size_t i = 0; i < NP; i++)
+            for (size_t i = 0; i < count; i++)
                 ((volatile uint32_t *)flags)[i] = 0;
-        if (reshaped_alias || !c->use_graphs)
+        if (!graphs)
         {
             c->graph_stats[Context_::GS_NO_GRAPH]++;
-            if (NP != N) // (this branch runs unpadded: second operands sit right behind the first N)
-                for (size_t i = 0; i < N && operands == 2; i++)
-                    tab[N + i] = const_cast<u64 *>(batch[i]->b->dev_ptr(c));
-            void *pin = nullptr, *pout = nullptr;
-            dev_check(b200_malloc_async(c->dev, operands * N * win * sizeof(u64), &pin, cur_stream()));
-            dev_check(b200_malloc_async(c->dev, N * wout * sizeof(u64), &pout, cur_stream()));
-            u64 *in = (u64 *)pin, *out = (u64 *)pout;
-            int rc = b200_gather_scatter_table(c->dev, tab, operands * N, in, win, 1, cur_stream());
-            if (!rc)
-                rc = r0.kind == 0   ? b200_multiply(c->dev, lv, in, 2, in + N * win, 2, out, N, cur_stream())
-                     : r0.kind == 1 ? b200_relinearize(c->dev, lv, in, key, out, N, cur_stream())
-                                    : b200_apply_galois(c->dev, lv, in, r0.elt, key, out, N, cur_stream());
-            for (size_t i = 0; i < N; i++)
-                dtab[i] = batch[i]->dst->prepare_output(c, c->ids[lv], out_polys, k);
-            if (!rc)
-                rc = b200_gather_scatter_table(c->dev, dtab, N, out, wout, 0, cur_stream());
-            if (!rc && c->check_transparent)
-                rc = b200_any_nonzero(c->dev, lv, out, (int)out_polys, flags, N, cur_stream());
-            b200_free_async(c->dev, pin, cur_stream());
-            b200_free_async(c->dev, pout, cur_stream());
-            dev_check(rc);
+            dev_check(sequence(prepare)); // prepared after the layer-1 call: an aliased operand is gathered before its release
         }
         else
         {
-            for (size_t i = 0; i < NP; i++)
-                dtab[i] = i < N ? batch[i]->dst->prepare_output(c, c->ids[lv], out_polys, k) : lane.pad_out;
+            prepare();
             Context_::Lane::Graph *g = nullptr;
             for (auto &e : lane.graphs)
-                if ((e.kind == r0.kind || e.kind == -1 - r0.kind) && e.lv == lv && e.n == NP && e.key == (const void *)key && e.elt == r0.elt)
+                if ((e.kind == r0.kind || e.kind == -1 - r0.kind) && e.lv == lv && e.n == count && e.key == (const void *)key && e.elt == r0.elt)
                     g = &e;
             if (!g)
             { // first sight of this shape on this lane: run it kernel by kernel (this also warms every cache the sequence touches)
@@ -287,7 +304,7 @@ static void combine_run_batch(Context_ *c, std::vector<CombineReq *> &batch)
                         b200_graph_destroy(c->dev, lane.graphs[old].exec);
                     lane.graphs.erase(lane.graphs.begin() + (long)old);
                 }
-                lane.graphs.push_back({ r0.kind, lv, NP, (const void *)key, nullptr, ++lane.clock, r0.elt });
+                lane.graphs.push_back({ r0.kind, lv, count, (const void *)key, nullptr, ++lane.clock, r0.elt });
                 dev_check(enqueue());
             }
             else
@@ -505,20 +522,48 @@ void relinearize_direct(Context_ *c, Ciphertext_ &a, KSwitchKeys_ &keys, Ciphert
     transparent_guard(c, lv, dst);
 }
 
-void op_galois(Context_ *c, Ciphertext_ &a, uint32_t elt, KSwitchKeys_ &keys, Ciphertext_ &dst)
+bool has_galois_key(const KSwitchKeys_ &keys, uint32_t elt)
 {
-    // caller holds c->mu
-    int lv = data_level(c, a, "encrypted is not valid for encryption parameters");
+    const size_t idx = (elt - 1) >> 1;
+    return idx < keys.keys.size() && !keys.keys[idx].empty();
+}
+// the key list's index of Galois element `elt`, whose key must be present
+size_t galois_key_index(Context_ *c, KSwitchKeys_ &keys, uint32_t elt)
+{
+    if (!has_galois_key(keys, elt))
+        throw InvalidArg("Galois key not present");
+    const size_t idx = (elt - 1) >> 1;
+    check_keys(c, keys, idx);
+    return idx;
+}
+// the Galois element of a row rotation by `step`
+uint32_t row_step_elt(Context_ *c, int step)
+{
+    uint32_t elt = 0;
+    if (b200_galois_elt_from_step(c->dev, step, &elt))
+        throw InvalidArg("step count too large");
+    return elt;
+}
+
+// the checks of apply_galois (S/evaluator.cpp), in its order: returns the level of `a` and the key list's index of `elt`
+std::pair<int, size_t> galois_checks(Context_ *c, Ciphertext_ &a, uint32_t elt, KSwitchKeys_ &keys)
+{
+    const int lv = data_level(c, a, "encrypted is not valid for encryption parameters");
     if (keys.parms_id != c->ids[0])
         throw InvalidArg("galois_keys is not valid for encryption parameters");
     if (!(elt & 1) || elt >= 2 * c->parms.n)
         throw InvalidArg("Galois element is not valid");
     if (a.size > 2)
         throw InvalidArg("encrypted size must be 2");
-    const size_t index = (elt - 1) >> 1;
-    if (index >= keys.keys.size() || keys.keys[index].empty())
-        throw InvalidArg("Galois key not present");
-    check_keys(c, keys, index);
+    return { lv, galois_key_index(c, keys, elt) };
+}
+
+void op_galois(Context_ *c, Ciphertext_ &a, uint32_t elt, KSwitchKeys_ &keys, Ciphertext_ &dst)
+{
+    // caller holds c->mu
+    int lv;
+    size_t index;
+    std::tie(lv, index) = galois_checks(c, a, elt, keys);
     const u64 *pa = a.dev_ptr(c);
     const u64 *key = keys.flat_dev(c, index, (int)a.k);
     with_output(c, dst, { &a }, a.parms_id, 2, a.k, [&](u64 *out) {
@@ -543,23 +588,33 @@ std::vector<int> naf(int value)
     return res;
 }
 
+// The Galois elements rotate_internal (S/evaluator.cpp:2325-2380) applies for a row rotation by `steps` != 0: the step's own
+// when its key is present, else those of its NAF parts, skipping the parts of +-n/2 (the identity on rows).  No part's
+// magnitude exceeds n/2, so every remaining part has an element.
+std::vector<uint32_t> row_rotation_elts(Context_ *c, const KSwitchKeys_ &keys, int steps)
+{
+    const uint32_t elt = row_step_elt(c, steps);
+    if (has_galois_key(keys, elt))
+        return { elt };
+    const std::vector<int> parts = naf(steps);
+    if (parts.size() == 1)
+        throw InvalidArg("Galois key not present");
+    std::vector<uint32_t> elts;
+    for (int st : parts)
+        if ((size_t)std::abs(st) != (c->parms.n >> 1))
+            elts.push_back(row_step_elt(c, st));
+    return elts;
+}
+
 // One application of a Galois automorphism whose key is present, through the combiner (same checks, same errors as op_galois);
 // false: not combinable here (combining off, nested call) — the caller takes the direct path.
 bool galois_combined(Context_ *c, Ciphertext_ &a, uint32_t elt, KSwitchKeys_ &keys, Ciphertext_ &dst)
 {
     if (!c->combine || tl_scope)
         return false;
-    int lv = data_level(c, a, "encrypted is not valid for encryption parameters");
-    if (keys.parms_id != c->ids[0])
-        throw InvalidArg("galois_keys is not valid for encryption parameters");
-    if (!(elt & 1) || elt >= 2 * c->parms.n)
-        throw InvalidArg("Galois element is not valid");
-    if (a.size > 2)
-        throw InvalidArg("encrypted size must be 2");
-    const size_t index = (elt - 1) >> 1;
-    if (index >= keys.keys.size() || keys.keys[index].empty())
-        throw InvalidArg("Galois key not present");
-    check_keys(c, keys, index);
+    int lv;
+    size_t index;
+    std::tie(lv, index) = galois_checks(c, a, elt, keys);
     if (keys.keys[index].size() < (size_t)a.k || a.is_ntt_form)
         return false; // let the direct path report it
     CombineReq r;
@@ -586,31 +641,17 @@ void op_rotate(Context_ *c, Ciphertext_ &a, int steps, KSwitchKeys_ &keys, Ciphe
         dst.assign(a);
         return;
     }
-    const size_t n = c->parms.n;
-    uint32_t elt = 0;
-    if (b200_galois_elt_from_step(c->dev, steps, &elt))
-        throw InvalidArg("step count too large");
-    auto has = [&](uint32_t e) {
-        size_t idx = (e - 1) >> 1;
-        return idx < keys.keys.size() && !keys.keys[idx].empty();
-    };
-    if (has(elt))
+    // A plan of one element applies the step's own element: the NAF {x, +-n/2} rotates by x, whose element is the step's.
+    const std::vector<uint32_t> elts = row_rotation_elts(c, keys, steps);
+    if (elts.size() == 1)
     {
-        op_galois(c, a, elt, keys, dst);
+        op_galois(c, a, elts[0], keys, dst);
         return;
     }
-    std::vector<int> parts = naf(steps);
-    if (parts.size() == 1)
-        throw InvalidArg("Galois key not present");
     Ciphertext_ cur;
     cur.assign(a);
-    for (int st : parts)
+    for (uint32_t e : elts)
     {
-        if ((size_t)std::abs(st) == (n >> 1))
-            continue; // a rotation by the full row is the identity
-        uint32_t e = 0;
-        if (b200_galois_elt_from_step(c->dev, st, &e))
-            throw InvalidArg("step count too large");
         Ciphertext_ nxt;
         op_galois(c, cur, e, keys, nxt);
         cur.assign(nxt);
@@ -638,21 +679,22 @@ std::vector<u64> padded_plain(Context_ *c, const Plaintext_ &p, bool check_value
     return v;
 }
 
+// The plaintext operand of an Evaluator operation, padded to n coefficients; multiplying by zero gives a transparent result
+std::vector<u64> plain_operand(Context_ *c, const Plaintext_ &p, bool multiply)
+{
+    std::vector<u64> v = padded_plain(c, p, false);
+    if (multiply && c->check_transparent && std::all_of(v.begin(), v.end(), [](u64 x) { return x == 0; }))
+        throw LogicErr("result ciphertext is transparent");
+    return v;
+}
+
 void op_plain(Context_ *c, Ciphertext_ &a, const Plaintext_ &p, Ciphertext_ &dst, int which /*0 add 1 sub 2 mul*/)
 {
     OpScope scope(c);
     int lv = data_level(c, a, "encrypted is not valid for encryption parameters");
     if (a.is_ntt_form)
         throw InvalidArg("BFV encrypted cannot be in NTT form");
-    std::vector<u64> pv = padded_plain(c, p, false);
-    if (which == 2)
-    {
-        bool zero = true;
-        for (u64 x : pv)
-            zero = zero && x == 0;
-        if (zero && c->check_transparent)
-            throw LogicErr("result ciphertext is transparent");
-    }
+    std::vector<u64> pv = plain_operand(c, p, which == 2);
     void *dp = nullptr;
     dev_check(b200_malloc(c->dev, pv.size() * sizeof(u64), &dp));
     int rc = b200_memcpy_h2d(c->dev, dp, pv.data(), pv.size() * sizeof(u64), cur_stream());
@@ -1985,12 +2027,9 @@ long Evaluator_RotateRows(void *p, void *a, int steps, void *keys, void *dst, vo
         if (c->combine && c->using_batching && K.parms_id == c->ids[0] && steps != 0)
         { // a rotation whose key is present is one key switch: concurrent ones are combined like multiply / relinearize
             uint32_t elt = 0;
-            if (b200_galois_elt_from_step(c->dev, steps, &elt) == 0)
-            {
-                const size_t idx = (elt - 1) >> 1;
-                if (idx < K.keys.size() && !K.keys[idx].empty() && galois_combined(c, *(Ciphertext_ *)a, elt, K, *(Ciphertext_ *)dst))
-                    return;
-            }
+            if (b200_galois_elt_from_step(c->dev, steps, &elt) == 0 && has_galois_key(K, elt) &&
+                galois_combined(c, *(Ciphertext_ *)a, elt, K, *(Ciphertext_ *)dst))
+                return;
         }
         OpScope scope(c);
         op_rotate(c, *(Ciphertext_ *)a, steps, K, *(Ciphertext_ *)dst);
@@ -2036,31 +2075,23 @@ void batch_handles(uint64_t count, std::initializer_list<void **> arrays)
         for (uint64_t i = 0; i < count; i++)
             NULLRET_THROW(arr[i]);
 }
-// slab words of one batch item, from the first (validated) handle
-u64 batch_item_words(Context_ *c, void **cts)
+// A batch seam's operation scope.  B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes.
+struct SeamScope : OpScope
 {
-    auto &a0 = *(Ciphertext_ *)cts[0];
-    data_level(c, a0, "encrypted is not valid for encryption parameters");
-    if (a0.size != 2 || a0.n != c->parms.n || a0.k == 0 || a0.k > c->parms.coeff.size())
-        throw InvalidArg("batch items must be size-2 ciphertexts at the same level");
-    return 2 * a0.k * c->parms.n;
+    explicit SeamScope(Context_ *c) : OpScope(c) { blocking = c->blocking_waits; }
+};
+// the Galois element of RotateRows(step) and its key list's index; a step without its own key is refused (no NAF parts)
+size_t row_step_key(Context_ *c, KSwitchKeys_ &keys, int step, uint32_t *elt)
+{
+    return galois_key_index(c, keys, *elt = row_step_elt(c, step));
 }
-int batch_gather(Context_ *c, uint64_t count, void **cts, BatchSlab &slab, u64 &k_out)
+// the items (checked by batch_level) one after the other in `slab`: one launch for all of them
+void batch_gather(Context_ *c, uint64_t count, void **cts, BatchSlab &slab)
 {
-    auto &a0 = *(Ciphertext_ *)cts[0];
-    const int lv = data_level(c, a0, "encrypted is not valid for encryption parameters");
-    const u64 w = 2 * a0.k * a0.n;
     std::vector<u64 *> ptrs(count);
     for (uint64_t i = 0; i < count; i++)
-    {
-        auto &a = *(Ciphertext_ *)cts[i];
-        if (data_level(c, a, "encrypted is not valid for encryption parameters") != lv || a.size != 2 || a.is_ntt_form)
-            throw InvalidArg("batch items must be size-2 ciphertexts at the same level");
-        ptrs[i] = const_cast<u64 *>(a.dev_ptr(c));
-    }
-    dev_check(b200_gather_scatter(c->dev, ptrs.data(), count, slab.w(), w, 1, cur_stream())); // one launch for all items
-    k_out = a0.k;
-    return lv;
+        ptrs[i] = const_cast<u64 *>(((Ciphertext_ *)cts[i])->dev_ptr(c));
+    dev_check(b200_gather_scatter(c->dev, ptrs.data(), count, slab.w(), ((Ciphertext_ *)cts[0])->words(), 1, cur_stream()));
 }
 void batch_scatter(Context_ *c, uint64_t count, void **dsts, const BatchSlab &slab, const ParmsId &id, u64 k, int level,
                    u64 size = 2)
@@ -2108,8 +2139,7 @@ long B200_Ciphertext_SetWordsBatch(void *context, uint64_t count, void **cts, ui
         if (count == 0)
             return;
         batch_handles(count, { cts });
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        SeamScope scope(c);
         const u64 k = (u64)c->level_k[lv];
         const u64 w = size * k * c->parms.n;
         BatchSlab S(c, count * w);
@@ -2140,8 +2170,7 @@ long B200_Ciphertext_GetWordsBatch(void *context, uint64_t count, void **cts, ui
         const u64 w = a0.words();
         if (cap < count * w)
             throw InvalidArg("capacity too small");
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        SeamScope scope(c);
         std::vector<u64 *> ptrs(count);
         for (uint64_t i = 0; i < count; i++)
         {
@@ -2244,14 +2273,14 @@ long B200_Evaluator_MultiplyRelinBatch(void *p, uint64_t count, void **e1, void 
         if (count == 0)
             return;
         batch_handles(count, { e1, e2, dsts });
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
-        const u64 w = batch_item_words(c, e1);
+        SeamScope scope(c);
+        const int lv = batch_level(c, count, e1);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * c->parms.n;
         BatchSlab A(c, count * w), B(c, count * w), D(c, count * w);
-        u64 k = 0, kb = 0;
-        const int lv = batch_gather(c, count, e1, A, k);
-        if (batch_gather(c, count, e2, B, kb) != lv)
+        batch_gather(c, count, e1, A);
+        if (batch_level(c, count, e2) != lv)
             throw InvalidArg("encrypted1 and encrypted2 parameter mismatch");
+        batch_gather(c, count, e2, B);
         check_keys(c, keys, 0);
         dev_check(b200_multiply_relin(c->dev, lv, A.w(), B.w(), keys.flat_dev(c, 0, (int)k), D.w(), count, cur_stream()));
         batch_scatter(c, count, dsts, D, ((Ciphertext_ *)e1[0])->parms_id, k, lv);
@@ -2268,14 +2297,14 @@ long B200_Evaluator_AddSubBatch(void *p, uint64_t count, void **e1, void **e2, b
         if (count == 0)
             return;
         batch_handles(count, { e1, e2, dsts });
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
-        const u64 w = batch_item_words(c, e1);
+        SeamScope scope(c);
+        const int lv = batch_level(c, count, e1);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * c->parms.n;
         BatchSlab A(c, count * w), B(c, count * w);
-        u64 k = 0, kb = 0;
-        const int lv = batch_gather(c, count, e1, A, k);
-        if (batch_gather(c, count, e2, B, kb) != lv)
+        batch_gather(c, count, e1, A);
+        if (batch_level(c, count, e2) != lv)
             throw InvalidArg("encrypted1 and encrypted2 parameter mismatch");
+        batch_gather(c, count, e2, B);
         dev_check((subtract ? b200_sub : b200_add)(c->dev, lv, A.w(), B.w(), A.w(), 2, count, cur_stream()));
         batch_scatter(c, count, dsts, A, ((Ciphertext_ *)e1[0])->parms_id, k, lv);
     });
@@ -2294,20 +2323,17 @@ long B200_Evaluator_PlainBatch(void *p, int which, uint64_t count, void **encs, 
         if (count == 0)
             return;
         batch_handles(count, { encs, plains, dsts });
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        SeamScope scope(c);
         const size_t n = c->parms.n;
-        const u64 w = batch_item_words(c, encs);
+        const int lv = batch_level(c, count, encs);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * n;
         BatchSlab A(c, count * w), O(c, count * w), P(c, count * n);
-        u64 k = 0;
-        const int lv = batch_gather(c, count, encs, A, k);
+        batch_gather(c, count, encs, A);
         std::vector<u64> host(count * n);
         for (uint64_t i = 0; i < count; i++)
         {
             NULLRET_THROW(plains[i]);
-            std::vector<u64> pv = padded_plain(c, *(Plaintext_ *)plains[i], false);
-            if (which == 2 && c->check_transparent && std::all_of(pv.begin(), pv.end(), [](u64 x) { return x == 0; }))
-                throw LogicErr("result ciphertext is transparent");
+            std::vector<u64> pv = plain_operand(c, *(Plaintext_ *)plains[i], which == 2);
             std::copy(pv.begin(), pv.end(), host.begin() + i * n);
         }
         dev_check(b200_memcpy_h2d(c->dev, P.p, host.data(), host.size() * 8, cur_stream()));
@@ -2336,26 +2362,20 @@ long B200_Evaluator_RotateRowsBatch(void *p, uint64_t count, void **encs, int st
         if (!c->using_batching)
             throw LogicErr("encryption parameters do not support batching");
         batch_handles(count, { encs, dsts });
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
-        const u64 w = batch_item_words(c, encs);
+        SeamScope scope(c);
+        const int lv = batch_level(c, count, encs);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * c->parms.n;
         BatchSlab A(c, count * w), O(c, count * w);
-        u64 k = 0;
-        const int lv = batch_gather(c, count, encs, A, k);
+        batch_gather(c, count, encs, A);
         if (steps == 0)
         {
             batch_scatter(c, count, dsts, A, ((Ciphertext_ *)encs[0])->parms_id, k, lv);
             return;
         }
-        uint32_t elt = 0;
-        if (b200_galois_elt_from_step(c->dev, steps, &elt))
-            throw InvalidArg("step count too large");
-        const size_t index = (elt - 1) >> 1;
+        const uint32_t elt = row_step_elt(c, steps);
         if (keys.parms_id != c->ids[0])
             throw InvalidArg("galois_keys is not valid for encryption parameters");
-        if (index >= keys.keys.size() || keys.keys[index].empty())
-            throw InvalidArg("Galois key not present");
-        check_keys(c, keys, index);
+        const size_t index = galois_key_index(c, keys, elt);
         dev_check(b200_apply_galois(c->dev, lv, A.w(), elt, keys.flat_dev(c, index, (int)k), O.w(), count, cur_stream()));
         batch_scatter(c, count, dsts, O, ((Ciphertext_ *)encs[0])->parms_id, k, lv);
     });
@@ -2380,8 +2400,7 @@ long B200_Evaluator_MultiplyPlainSum(void *p, uint64_t rows, uint64_t cols, void
         batch_handles(cols, { encs });
         batch_handles(rows, { dsts });
         batch_handles(rows * cols, { plains });
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
+        SeamScope scope(c);
         const size_t n = c->parms.n;
         auto &a0 = *(Ciphertext_ *)encs[0];
         const int lv = data_level(c, a0, "encrypted is not valid for encryption parameters");
@@ -2403,9 +2422,7 @@ long B200_Evaluator_MultiplyPlainSum(void *p, uint64_t rows, uint64_t cols, void
         std::vector<u64> host(rows * cols * n);
         for (uint64_t i = 0; i < rows * cols; i++)
         {
-            std::vector<u64> pv = padded_plain(c, *(Plaintext_ *)plains[i], false);
-            if (c->check_transparent && std::all_of(pv.begin(), pv.end(), [](u64 x) { return x == 0; }))
-                throw LogicErr("result ciphertext is transparent");
+            std::vector<u64> pv = plain_operand(c, *(Plaintext_ *)plains[i], true);
             std::copy(pv.begin(), pv.end(), host.begin() + i * n);
         }
         BatchSlab X(c, cols * w);
@@ -2481,17 +2498,15 @@ long B200_Evaluator_MultiplyRelinSum(void *p, uint64_t rows, uint64_t cols, void
                 throw InvalidArg("kswitch_keys is not valid for encryption parameters");
             same = same && e1[t] == e2[t];
         }
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
-        const u64 w = batch_item_words(c, e1);
+        SeamScope scope(c);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * c->parms.n;
         BatchSlab A(c, terms * w);
         std::unique_ptr<BatchSlab> B;
-        u64 k = 0, kb = 0;
-        batch_gather(c, terms, e1, A, k);
+        batch_gather(c, terms, e1, A);
         if (!same)
         {
             B.reset(new BatchSlab(c, terms * w));
-            batch_gather(c, terms, e2, *B, kb);
+            batch_gather(c, terms, e2, *B);
         }
         const u64 *pb = same ? A.w() : B->w();
         if (c->check_transparent)
@@ -2549,58 +2564,30 @@ long B200_Evaluator_RotateSumBatch(void *p, uint64_t count, void **encs, int nst
         if (keys.parms_id != c->ids[0])
             throw InvalidArg("galois_keys is not valid for encryption parameters");
         const size_t n = c->parms.n;
-        auto key_index = [&](uint32_t e) -> size_t {
-            const size_t idx = (e - 1) >> 1;
-            if (idx >= keys.keys.size() || keys.keys[idx].empty())
-                throw InvalidArg("Galois key not present");
-            check_keys(c, keys, idx);
-            return idx;
-        };
-        auto elt_of = [&](int st) {
-            uint32_t e = 0;
-            if (b200_galois_elt_from_step(c->dev, st, &e))
-                throw InvalidArg("step count too large");
-            return e;
-        };
         // per step, the Galois elements the chain applies (empty: c + c)
         std::vector<std::vector<uint32_t>> plan;
         for (int i = 0; i < nsteps; i++)
         {
             std::vector<uint32_t> elts;
             if (steps[i] != 0)
-            {
-                const uint32_t e = elt_of(steps[i]);
-                const size_t idx = (e - 1) >> 1;
-                if (idx < keys.keys.size() && !keys.keys[idx].empty())
-                    elts.push_back(e);
-                else
-                {
-                    const std::vector<int> parts = naf(steps[i]);
-                    if (parts.size() == 1)
-                        throw InvalidArg("Galois key not present");
-                    for (int st : parts)
-                        if ((size_t)std::abs(st) != (n >> 1))
-                            elts.push_back(elt_of(st));
-                }
-                for (uint32_t x : elts)
-                    key_index(x);
-            }
+                elts = row_rotation_elts(c, keys, steps[i]);
+            for (uint32_t x : elts)
+                galois_key_index(c, keys, x);
             plan.push_back(std::move(elts));
         }
         if (columns)
         {
-            key_index((uint32_t)(2 * n - 1));
+            galois_key_index(c, keys, (uint32_t)(2 * n - 1));
             plan.push_back({ (uint32_t)(2 * n - 1) });
         }
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
-        const u64 w = batch_item_words(c, encs);
+        SeamScope scope(c);
+        const int lv = batch_level(c, count, encs);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * n;
         BatchSlab A(c, count * w), B(c, count * w);
         std::unique_ptr<BatchSlab> T; // third slab for NAF steps of three or more parts
-        u64 k = 0;
-        const int lv = batch_gather(c, count, encs, A, k);
+        batch_gather(c, count, encs, A);
         BatchSlab *cur = &A, *other = &B;
-        auto key = [&](uint32_t e) { return keys.flat_dev(c, key_index(e), (int)k); };
+        auto key = [&](uint32_t e) { return keys.flat_dev(c, galois_key_index(c, keys, e), (int)k); };
         for (const auto &elts : plan)
         {
             if (elts.empty())
@@ -2630,21 +2617,6 @@ long B200_Evaluator_RotateSumBatch(void *p, uint64_t count, void **encs, int nst
     });
 }
 
-namespace
-{
-// the Galois element of RotateRows(step) and its key list's index; a step without its own key is refused (no NAF parts)
-size_t row_step_key(Context_ *c, KSwitchKeys_ &keys, int step, uint32_t *elt)
-{
-    if (b200_galois_elt_from_step(c->dev, step, elt))
-        throw InvalidArg("step count too large");
-    const size_t idx = (*elt - 1) >> 1;
-    if (idx >= keys.keys.size() || keys.keys[idx].empty())
-        throw InvalidArg("Galois key not present");
-    check_keys(c, keys, idx);
-    return idx;
-}
-} // namespace
-
 // Row rotations by a step per item.  The items are gathered in the order of their Galois elements (step 0 last, a copy), so
 // each element's items are one run of one key, and rotated by one b200_apply_galois_many; the results are scattered back to
 // their destinations.  Every operand is gathered before the scatter, so destinations may alias encrypteds.
@@ -2663,14 +2635,7 @@ long B200_Evaluator_RotateRowsStepsBatch(void *p, uint64_t count, void **encs, c
         if (!c->using_batching)
             throw LogicErr("encryption parameters do not support batching");
         batch_handles(count, { encs, dsts });
-        batch_item_words(c, encs);
-        for (uint64_t i = 0; i < count; i++)
-        {
-            auto &a = *(Ciphertext_ *)encs[i];
-            data_level(c, a, "encrypted is not valid for encryption parameters");
-            if (a.is_ntt_form || a.size != 2)
-                throw InvalidArg("batch items must be size-2 ciphertexts at the same level");
-        }
+        const int lv = batch_level(c, count, encs);
         if (!c->using_keyswitching)
             throw LogicErr("keyswitching is not supported by the context");
         if (keys.parms_id != c->ids[0])
@@ -2695,12 +2660,10 @@ long B200_Evaluator_RotateRowsStepsBatch(void *p, uint64_t count, void **encs, c
         uint64_t m = 0; // items with a rotation
         while (m < count && elt[order[m]])
             m++;
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
-        const u64 w = batch_item_words(c, encs);
+        SeamScope scope(c);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * c->parms.n;
         BatchSlab A(c, count * w), O(c, count * w);
-        u64 k = 0;
-        const int lv = batch_gather(c, count, src.data(), A, k);
+        batch_gather(c, count, src.data(), A);
         if (m)
         {
             std::vector<uint32_t> el(m);
@@ -2740,14 +2703,9 @@ long B200_Evaluator_LinearTransform(void *p, uint64_t count, void **encs, uint64
         if (!c->using_batching)
             throw LogicErr("encryption parameters do not support batching");
         batch_handles(count, { encs, dsts });
-        batch_item_words(c, encs);
+        // each item on its own: items at different levels are refused after the plaintexts (a zero one is a LogicErr)
         for (uint64_t i = 0; i < count; i++)
-        {
-            auto &a = *(Ciphertext_ *)encs[i];
-            data_level(c, a, "encrypted is not valid for encryption parameters");
-            if (a.is_ntt_form || a.size != 2)
-                throw InvalidArg("batch items must be size-2 ciphertexts at the same level");
-        }
+            batch_level(c, 1, encs + i);
         const size_t n = c->parms.n;
         const uint64_t terms = baby * giant;
         std::vector<uint8_t> present(terms, 0);
@@ -2757,9 +2715,7 @@ long B200_Evaluator_LinearTransform(void *p, uint64_t count, void **encs, uint64
         {
             if (!plains[t])
                 continue;
-            std::vector<u64> pv = padded_plain(c, *(Plaintext_ *)plains[t], false);
-            if (c->check_transparent && std::all_of(pv.begin(), pv.end(), [](u64 x) { return x == 0; }))
-                throw LogicErr("result ciphertext is transparent");
+            std::vector<u64> pv = plain_operand(c, *(Plaintext_ *)plains[t], true);
             std::copy(pv.begin(), pv.end(), host.begin() + t * n);
             present[t] = 1;
             ub[t % baby] = ug[t / baby] = 1;
@@ -2791,12 +2747,11 @@ long B200_Evaluator_LinearTransform(void *p, uint64_t count, void **encs, uint64
                     throw InvalidArg("step count too large");
                 idx[baby - 1 + g - 1] = row_step_key(c, keys, (int)(g * baby), &elts[baby - 1 + g - 1]);
             }
-        OpScope scope(c);
-        scope.blocking = c->blocking_waits; // B200_BLOCKING_WAITS=1: sleep instead of spinning while the batch completes
-        const u64 w = batch_item_words(c, encs);
+        SeamScope scope(c);
+        const int lv = batch_level(c, count, encs);
+        const u64 k = (u64)c->level_k[lv], w = 2 * k * n;
         BatchSlab A(c, count * w), O(c, count * w);
-        u64 k = 0;
-        const int lv = batch_gather(c, count, encs, A, k);
+        batch_gather(c, count, encs, A);
         std::vector<const uint64_t *> kp(std::max<uint64_t>(ns, 1), nullptr);
         for (uint64_t e = 0; e < ns; e++)
             if (elts[e])

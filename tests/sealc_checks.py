@@ -1125,6 +1125,9 @@ def misuse_hresults(S, n, moduli, t):
     both("RotateRows with relinearization keys", lambda L, o: L.rc("Evaluator_RotateRows", o["ev"], o["ct"], C.c_int(1), o["rlk"], o["dst"], None))
     both("RotateRows by 0", lambda L, o: (L.rc("Evaluator_RotateRows", o["ev"], o["ct"], C.c_int(0), o["rlk"], o["dst"], None),))
     both("RotateRows by n", lambda L, o: L.rc("Evaluator_RotateRows", o["ev"], o["ct"], C.c_int(n), o["rlk"], o["dst"], None))
+    both("RotateRows with an empty key object", lambda L, o: L.rc("Evaluator_RotateRows", o["ev"], o["ct"], C.c_int(1), L.new("KSwitchKeys"), o["dst"], None))
+    both("RotateColumns with an empty key object", lambda L, o: L.rc("Evaluator_RotateColumns", o["ev"], o["ct"], L.new("KSwitchKeys"), o["dst"], None))
+    both("ApplyGalois of an even element", lambda L, o: L.rc("Evaluator_ApplyGalois", o["ev"], o["ct"], C.c_uint32(2), o["rlk"], o["dst"], None))
     both("Exponentiate to the power 0", lambda L, o: L.rc("Evaluator_Exponentiate", o["ev"], o["ct"], u64(0), o["rlk"], o["dst"], None))
     both("Exponentiate to the power 1", lambda L, o: (L.rc("Evaluator_Exponentiate", o["ev"], o["ct"], u64(1), o["rlk"], o["dst"], None), L.save("Ciphertext", o["dst"], 0)))
     both("MultiplyMany of nothing", lambda L, o: L.rc("Evaluator_MultiplyMany", o["ev"], u64(0), (vp * 1)(), o["rlk"], o["dst"], None))

@@ -681,6 +681,9 @@ def seam_checks(S, params):
     assert lt_seam(S, O, octs, b, G, op, ogk, [None] + fresh(2)) == E_INVALIDARG
     zero = O.new_pt(np.zeros(1, dtype=np.uint64))
     assert lt_seam(S, O, octs, b, G, [zero] + op[1:], ogk, fresh()) == COR_E_INVALIDOPERATION   # MultiplyPlain by zero
+    if len(R.data_parms_ids()) > 1:  # the plaintexts are checked before the items' levels are compared
+        assert lt_seam(S, O, [octs[0], low], b, G, [zero] + op[1:], ogk, fresh(2)) == COR_E_INVALIDOPERATION
+        assert steps_batch(S, O, [octs[0], low], [1, 4], ogk, fresh(2)) == E_INVALIDARG
     # a trivial encryption (c1 = 0): the chain's rotations are transparent, the seam's final result too
     tr = O.ct_words(octs[0])
     tr[1] = 0
