@@ -207,7 +207,6 @@ int b200_any_nonzero(b200_ctx *ctx, int level, const uint64_t *ct, int size, uin
         H2D / compute / D2H are chunked and overlapped on internal streams; returns after completion ---- */
 int b200_multiply_relin_host(b200_ctx *ctx, int level, const uint64_t *a_host, const uint64_t *b_host,
                              const uint64_t *relin_key_dev, uint64_t *out_host, uint64_t batch);
-int b200_ntt_roundtrip_host(b200_ctx *ctx, int level, const uint64_t *in_host, uint64_t *out_host, uint64_t items);
 
 /* gather (`gather` != 0: slab[i*words..] <- *host_ptrs[i]) or scatter (*host_ptrs[i] <- slab[i*words..]) of `count` device
    buffers of `words` words in one launch; `host_ptrs` is a HOST array of device pointers and must stay valid until the

@@ -1243,6 +1243,159 @@ struct FpMasks
     int running = 0; // the schedule whose masks the transforms use
 };
 
+// minimal fork-join pool (the packing loops are pure streaming work; 8-16 threads saturate what PCIe can take)
+struct HostPool
+{
+    std::vector<std::thread> th;
+    std::mutex mu;
+    std::condition_variable cv_work, cv_done;
+    std::function<void(int, int)> task;
+    long long generation = 0;
+    int pending = 0;
+    bool stop = false;
+    int nth = 1;
+    explicit HostPool(int n) : nth(n < 1 ? 1 : n)
+    {
+        for (int i = 1; i < nth; i++)
+            th.emplace_back([this, i] { loop(i); });
+    }
+    ~HostPool()
+    {
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            stop = true;
+        }
+        cv_work.notify_all();
+        for (auto &t : th)
+            t.join();
+    }
+    void loop(int id)
+    {
+        long long seen = 0;
+        for (;;)
+        {
+            std::function<void(int, int)> fn;
+            {
+                std::unique_lock<std::mutex> lk(mu);
+                cv_work.wait(lk, [&] { return stop || generation != seen; });
+                if (stop)
+                    return;
+                seen = generation;
+                fn = task;
+            }
+            fn(id, nth);
+            {
+                std::lock_guard<std::mutex> lk(mu);
+                if (--pending == 0)
+                    cv_done.notify_one();
+            }
+        }
+    }
+    void run(const std::function<void(int, int)> &fn)
+    {
+        if (nth == 1)
+        {
+            fn(0, 1);
+            return;
+        }
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            task = fn;
+            pending = nth - 1;
+            generation++;
+        }
+        cv_work.notify_all();
+        fn(0, nth);
+        std::unique_lock<std::mutex> lk(mu);
+        cv_done.wait(lk, [&] { return pending == 0; });
+    }
+};
+
+// `destroy(h)` when `h` was created; `h` is null afterwards
+template <class H, class F>
+static void release(H &h, F destroy)
+{
+    if (h)
+        destroy(h);
+    h = nullptr;
+}
+
+// Staging ring of the host-buffer entry points: NBUF slots, each with device buffers for both operands and the result and the
+// events that mark its copy-in, compute and copy-out, plus the packed staging (6 bytes per word, see level_packs): pinned host
+// buffers and device landing zones.  Allocated on first use and grown, never shrunk; released with the context.
+struct StagingRing
+{
+    static const int NBUF = 3;
+    struct Slot
+    {
+        u64 *a = nullptr, *b = nullptr, *o = nullptr;
+        cudaEvent_t in = nullptr, comp = nullptr, out = nullptr;
+        uint8_t *hst_a = nullptr, *hst_b = nullptr, *hst_o = nullptr;
+        u64 *dpk_a = nullptr, *dpk_b = nullptr, *dpk_o = nullptr;
+    } slot[NBUF];
+    size_t words = 0, pk_words = 0; // words per slot the plain / packed buffers hold (0 until an allocation round succeeded)
+    std::mutex mu;                  // one host pipeline at a time
+
+    int reserve(size_t w)
+    {
+        if (words >= w)
+            return 0;
+        free_plain();
+        for (Slot &s : slot)
+        {
+            for (cudaEvent_t *e : { &s.in, &s.comp, &s.out })
+                if (!*e)
+                    CU_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+            for (u64 **p : { &s.a, &s.b, &s.o })
+                CU_TRY(cudaMalloc((void **)p, w * sizeof(u64)));
+        }
+        words = w;
+        return 0;
+    }
+    int reserve_packed(size_t w)
+    {
+        if (pk_words >= w)
+            return 0;
+        free_packed();
+        const size_t bytes = w * 6 + 16;
+        for (Slot &s : slot)
+        {
+            for (uint8_t **p : { &s.hst_a, &s.hst_b, &s.hst_o })
+                CU_TRY(cudaMallocHost((void **)p, bytes));
+            for (u64 **p : { &s.dpk_a, &s.dpk_b, &s.dpk_o })
+                CU_TRY(cudaMalloc((void **)p, bytes));
+        }
+        pk_words = w;
+        return 0;
+    }
+    void free_plain()
+    {
+        words = 0;
+        for (Slot &s : slot)
+            for (u64 **p : { &s.a, &s.b, &s.o })
+                release(*p, cudaFree);
+    }
+    void free_packed()
+    {
+        pk_words = 0;
+        for (Slot &s : slot)
+        {
+            for (uint8_t **p : { &s.hst_a, &s.hst_b, &s.hst_o })
+                release(*p, cudaFreeHost);
+            for (u64 **p : { &s.dpk_a, &s.dpk_b, &s.dpk_o })
+                release(*p, cudaFree);
+        }
+    }
+    ~StagingRing()
+    {
+        free_plain();
+        free_packed();
+        for (Slot &s : slot)
+            for (cudaEvent_t *e : { &s.in, &s.comp, &s.out })
+                release(*e, cudaEventDestroy);
+    }
+};
+
 struct b200_ctx
 {
     std::vector<LevelFpHost> fp_levels; // indexed like `levels`; empty tables when the level is not on the FP64 path
@@ -1253,7 +1406,7 @@ struct b200_ctx
     int ks_clusters[9] = {}; // [k]: k-CTA clusters of ks_cluster_kernel the device holds at once (0: no cluster kernel)
     size_t n = 0;
     int logn = 0;
-    std::vector<void *> allocations; // everything freed at destroy
+    std::vector<void *> allocations; // device tables (upload)
     NttPrime *d_ntt_primes = nullptr;
     NttPrimeFp *d_fp_primes = nullptr;
     bool fp_enabled = false;
@@ -1263,7 +1416,6 @@ struct b200_ctx
     int plain_prime_idx = -1;    // index of the plain modulus in the device prime tables (-1: no batching)
     PrimeDev *d_primes = nullptr;       // [all primes] key primes first
     std::vector<LevelDev> levels;       // device pointers inside
-    std::vector<const u64 *> d_inv_qlast; // per level
     const u64 *d_inv_qsp = nullptr;     // key level's inv_qlast: q_sp^-1 mod q_i
     int npass = 0;
     int pass_L[8];
@@ -1281,20 +1433,28 @@ struct b200_ctx
     cudaStream_t s_side[NSIDE] = { nullptr, nullptr, nullptr, nullptr };
     cudaEvent_t ev_fork = nullptr, ev_join[NSIDE] = { nullptr, nullptr, nullptr, nullptr };
     int mr_split = 1;
-    // staging ring of the *_host entry points (allocated on first use, reused afterwards)
-    static const int NBUF = 3;
-    u64 *hp_a[NBUF] = { nullptr, nullptr, nullptr }, *hp_b[NBUF] = { nullptr, nullptr, nullptr }, *hp_o[NBUF] = { nullptr, nullptr, nullptr };
-    cudaEvent_t hp_in[NBUF], hp_comp[NBUF], hp_out[NBUF];
-    size_t hp_words = 0;
-    std::mutex hp_mu;
-    // packed (6 bytes per word) PCIe staging of the host-buffer entry points: pinned host buffers and device landing zones
-    uint8_t *hst_a[NBUF] = { nullptr, nullptr, nullptr }, *hst_b[NBUF] = { nullptr, nullptr, nullptr }, *hst_o[NBUF] = { nullptr, nullptr, nullptr };
-    u64 *dpk_a[NBUF] = { nullptr, nullptr, nullptr }, *dpk_b[NBUF] = { nullptr, nullptr, nullptr }, *dpk_o[NBUF] = { nullptr, nullptr, nullptr };
-    size_t pk_words = 0;
-    struct HostPool *pool = nullptr;
+    StagingRing ring;
+    std::unique_ptr<HostPool> pool; // packing threads of the packed staging (created on first use)
     int ntt_threads = 256;
     size_t ntt_smem = 0;
     int ntt_split = 0; // n > 16384: two-level transform, ntt_outer_kernel + 2^split sub-transforms of n >> split points
+
+    // Releases what was created and makes no runtime call for what was not, so it also undoes a create that failed part-way
+    // (or before it reached the device).  b200_ctx_destroy synchronises first; a failed create has no work in flight.
+    ~b200_ctx()
+    {
+        for (void *p : allocations)
+            cudaFree(p);
+        for (int i = 0; i < NSIDE; i++)
+        {
+            release(s_side[i], cudaStreamDestroy);
+            release(ev_join[i], cudaEventDestroy);
+        }
+        release(ev_fork, cudaEventDestroy);
+        for (cudaStream_t *s : { &s_alloc, &s_h2d, &s_comp, &s_d2h })
+            release(*s, cudaStreamDestroy);
+        release(mempool, cudaMemPoolDestroy);
+    }
 };
 
 template <class T>
@@ -1460,7 +1620,6 @@ static int build_device(b200_ctx *ctx)
         PrimeDev *dbsk = nullptr;
         UP(bsk, &dbsk);
         L.bsk = dbsk;
-        L.m_sk = H.primes[H.aux0].mod.p;
         L.t = H.t;
         L.t_mod = prime_dev(H.t_mod);
         L.gamma = pd[Lh.gamma_idx];
@@ -1472,19 +1631,6 @@ static int build_device(b200_ctx *ctx)
         UP(_v, &d);                                                                                                    \
         L.field = d;                                                                                                   \
     } while (0)
-        UPF(lift_c, flat(Lh.lift_c));
-        UPF(lift_mat, Lh.lift_mat);
-        UPF(lift_mt, Lh.lift_mt);
-        UPF(lift_qm, Lh.lift_qm);
-        L.neg_inv_q_mod_mt = Lh.neg_inv_q_mod_mt;
-        UPF(scale_c, flat(Lh.scale_c));
-        UPF(scale_tq, Lh.scale_tq);
-        UPF(scale_mat, Lh.scale_mat);
-        UPF(sk_c, flat(Lh.sk_c));
-        UPF(sk_mat_q, Lh.sk_mat_q);
-        UPF(sk_mat_msk, Lh.sk_mat_msk);
-        UPF(sk_prod_b_q, Lh.sk_prod_b_q);
-        L.sk_inv_b_msk = Lh.sk_inv_b_msk;
         UPF(inv_qlast, flat(Lh.inv_qlast));
         UPF(delta, Lh.delta);
         UPF(plain_inc, Lh.plain_upper_half_inc);
@@ -2430,46 +2576,12 @@ int b200_ctx_create(uint64_t n, const uint64_t *coeff_modulus, uint64_t count, u
     return 0;
 }
 
-static void host_pool_destroy(b200_ctx *ctx);
 void b200_ctx_destroy(b200_ctx *ctx)
 {
     if (!ctx)
         return;
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
-    for (void *p : ctx->allocations)
-        cudaFree(p);
-    for (int i = 0; i < b200_ctx::NBUF; i++)
-        if (ctx->hst_a[i])
-        {
-            cudaFreeHost(ctx->hst_a[i]);
-            cudaFreeHost(ctx->hst_b[i]);
-            cudaFreeHost(ctx->hst_o[i]);
-            cudaFree(ctx->dpk_a[i]);
-            cudaFree(ctx->dpk_b[i]);
-            cudaFree(ctx->dpk_o[i]);
-        }
-    host_pool_destroy(ctx); // (HostPool is defined further down: deleting it here would delete an incomplete type)
-    for (int i = 0; i < b200_ctx::NBUF; i++)
-        if (ctx->hp_a[i])
-        {
-            cudaFree(ctx->hp_a[i]);
-            cudaFree(ctx->hp_b[i]);
-            cudaFree(ctx->hp_o[i]);
-            cudaEventDestroy(ctx->hp_in[i]);
-            cudaEventDestroy(ctx->hp_comp[i]);
-            cudaEventDestroy(ctx->hp_out[i]);
-        }
-    if (ctx->s_alloc)
-        cudaStreamDestroy(ctx->s_alloc);
-    if (ctx->s_h2d)
-        cudaStreamDestroy(ctx->s_h2d);
-    if (ctx->s_comp)
-        cudaStreamDestroy(ctx->s_comp);
-    if (ctx->s_d2h)
-        cudaStreamDestroy(ctx->s_d2h);
-    if (ctx->mempool)
-        cudaMemPoolDestroy(ctx->mempool);
     delete ctx;
 }
 
@@ -4025,32 +4137,19 @@ int b200_any_nonzero(b200_ctx *ctx, int level, const uint64_t *ct, int size, uin
 }
 
 // ---- host-buffer variants ----
-static int host_ring(b200_ctx *ctx, size_t words_per_slot)
+// end of a host pipeline: wait for its three streams; the loop's own error `rc` comes first, then a stream's
+static int finish_host_pipeline(b200_ctx *ctx, int rc)
 {
-    if (ctx->hp_words >= words_per_slot)
-        return 0;
-    for (int i = 0; i < b200_ctx::NBUF; i++)
-    {
-        if (ctx->hp_a[i])
-        {
-            cudaFree(ctx->hp_a[i]);
-            cudaFree(ctx->hp_b[i]);
-            cudaFree(ctx->hp_o[i]);
-        }
-        else
-        {
-            CU_TRY(cudaEventCreateWithFlags(&ctx->hp_in[i], cudaEventDisableTiming));
-            CU_TRY(cudaEventCreateWithFlags(&ctx->hp_comp[i], cudaEventDisableTiming));
-            CU_TRY(cudaEventCreateWithFlags(&ctx->hp_out[i], cudaEventDisableTiming));
-        }
-        CU_TRY(cudaMalloc((void **)&ctx->hp_a[i], words_per_slot * sizeof(u64)));
-        CU_TRY(cudaMalloc((void **)&ctx->hp_b[i], words_per_slot * sizeof(u64)));
-        CU_TRY(cudaMalloc((void **)&ctx->hp_o[i], words_per_slot * sizeof(u64)));
-    }
-    ctx->hp_words = words_per_slot;
+    cudaError_t e1 = cudaStreamSynchronize(ctx->s_h2d);
+    cudaError_t e2 = cudaStreamSynchronize(ctx->s_comp);
+    cudaError_t e3 = cudaStreamSynchronize(ctx->s_d2h);
+    if (rc)
+        return rc;
+    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
+        return fail(B200_E_CUDA, std::string("host pipeline: ") +
+                                     cudaGetErrorString(e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3)));
     return 0;
 }
-
 
 // ---------------------------------------------------------------------------------------------------------
 // Packed PCIe transfers for the host-buffer entry points (OPT-IN, see level_packs).  A canonical residue of a level
@@ -4085,79 +4184,6 @@ __global__ void pack48_kernel(const u64 *in, u64 *packed, long long groups)
     packed[3 * g + 2] = (w2 >> 32) | (w3 << 16);
 }
 
-// minimal fork-join pool (the packing loops are pure streaming work; 8-16 threads saturate what PCIe can take)
-struct HostPool
-{
-    std::vector<std::thread> th;
-    std::mutex mu;
-    std::condition_variable cv_work, cv_done;
-    std::function<void(int, int)> task;
-    long long generation = 0;
-    int pending = 0;
-    bool stop = false;
-    int nth = 1;
-    explicit HostPool(int n) : nth(n < 1 ? 1 : n)
-    {
-        for (int i = 1; i < nth; i++)
-            th.emplace_back([this, i] { loop(i); });
-    }
-    ~HostPool()
-    {
-        {
-            std::lock_guard<std::mutex> lk(mu);
-            stop = true;
-        }
-        cv_work.notify_all();
-        for (auto &t : th)
-            t.join();
-    }
-    void loop(int id)
-    {
-        long long seen = 0;
-        for (;;)
-        {
-            std::function<void(int, int)> fn;
-            {
-                std::unique_lock<std::mutex> lk(mu);
-                cv_work.wait(lk, [&] { return stop || generation != seen; });
-                if (stop)
-                    return;
-                seen = generation;
-                fn = task;
-            }
-            fn(id, nth);
-            {
-                std::lock_guard<std::mutex> lk(mu);
-                if (--pending == 0)
-                    cv_done.notify_one();
-            }
-        }
-    }
-    void run(const std::function<void(int, int)> &fn)
-    {
-        if (nth == 1)
-        {
-            fn(0, 1);
-            return;
-        }
-        {
-            std::lock_guard<std::mutex> lk(mu);
-            task = fn;
-            pending = nth - 1;
-            generation++;
-        }
-        cv_work.notify_all();
-        fn(0, nth);
-        std::unique_lock<std::mutex> lk(mu);
-        cv_done.wait(lk, [&] { return pending == 0; });
-    }
-};
-
-static void host_pool_destroy(b200_ctx *ctx)
-{
-    delete ctx->pool;
-    ctx->pool = nullptr;
-}
 static HostPool *host_pool(b200_ctx *ctx)
 {
     if (!ctx->pool)
@@ -4172,9 +4198,9 @@ static HostPool *host_pool(b200_ctx *ctx)
             int avail = sched_getaffinity(0, sizeof(set), &set) == 0 ? CPU_COUNT(&set) : (int)std::thread::hardware_concurrency();
             n = std::max(1, std::min(16, avail / 2));
         }
-        ctx->pool = new HostPool(n);
+        ctx->pool.reset(new HostPool(n));
     }
-    return ctx->pool;
+    return ctx->pool.get();
 }
 
 // src[words] -> dst[6*words (+2 slack)]; returns the OR of all words (to verify that they fit 48 bits)
@@ -4231,99 +4257,67 @@ static bool level_packs(const b200_ctx *ctx, int level)
     return true;
 }
 
-static int pack_ring(b200_ctx *ctx, size_t words_per_slot)
-{
-    if (ctx->pk_words >= words_per_slot)
-        return 0;
-    const size_t bytes = words_per_slot * 6 + 16;
-    for (int i = 0; i < b200_ctx::NBUF; i++)
-    {
-        if (ctx->hst_a[i])
-        {
-            cudaFreeHost(ctx->hst_a[i]);
-            cudaFreeHost(ctx->hst_b[i]);
-            cudaFreeHost(ctx->hst_o[i]);
-            cudaFree(ctx->dpk_a[i]);
-            cudaFree(ctx->dpk_b[i]);
-            cudaFree(ctx->dpk_o[i]);
-        }
-        CU_TRY(cudaMallocHost((void **)&ctx->hst_a[i], bytes));
-        CU_TRY(cudaMallocHost((void **)&ctx->hst_b[i], bytes));
-        CU_TRY(cudaMallocHost((void **)&ctx->hst_o[i], bytes));
-        CU_TRY(cudaMalloc((void **)&ctx->dpk_a[i], bytes));
-        CU_TRY(cudaMalloc((void **)&ctx->dpk_b[i], bytes));
-        CU_TRY(cudaMalloc((void **)&ctx->dpk_o[i], bytes));
-    }
-    ctx->pk_words = words_per_slot;
-    return 0;
-}
-
 // multiply+relinearize over host buffers with packed transfers (see above); same contract as the plain pipeline
 static int multiply_relin_host_packed(b200_ctx *ctx, int level, const u64 *a_host, const u64 *b_host, const u64 *relin_key_dev,
                                       u64 *out_host, uint64_t batch, long long chunk, size_t ct_words)
 {
+    StagingRing &R = ctx->ring;
     int rc = 0;
-    if ((rc = host_ring(ctx, (size_t)chunk * ct_words)) || (rc = pack_ring(ctx, (size_t)chunk * ct_words)))
+    if ((rc = R.reserve((size_t)chunk * ct_words)) || (rc = R.reserve_packed((size_t)chunk * ct_words)))
         return rc;
     HostPool *pool = host_pool(ctx);
-    const int NBUF = b200_ctx::NBUF, LAG = NBUF - 1;
+    const int NBUF = StagingRing::NBUF, LAG = NBUF - 1;
     std::vector<uint64_t> offs;
     for (uint64_t off = 0; off < batch; off += (uint64_t)chunk)
         offs.push_back(off);
     const int iters = (int)offs.size();
     auto drain = [&](int j) { // bring the result of iteration j home
-        const int sl = j % NBUF;
+        const StagingRing::Slot &S = R.slot[j % NBUF];
         const size_t words = (size_t)std::min<uint64_t>((uint64_t)chunk, batch - offs[j]) * ct_words;
-        cudaEventSynchronize(ctx->hp_out[sl]);
-        cpu_unpack48(pool, ctx->hst_o[sl], out_host + offs[j] * ct_words, words);
+        cudaEventSynchronize(S.out);
+        cpu_unpack48(pool, S.hst_o, out_host + offs[j] * ct_words, words);
     };
     u64 ormask = 0;
     for (int it = 0; it < iters && rc == 0; it++)
     {
-        const int sl = it % NBUF;
+        StagingRing::Slot &S = R.slot[it % NBUF];
         const uint64_t off = offs[it];
         const long long cnt = (long long)std::min<uint64_t>((uint64_t)chunk, batch - off);
         const size_t words = (size_t)cnt * ct_words, pbytes = words * 6, groups = words / 4;
         if (it >= NBUF)
-            cudaEventSynchronize(ctx->hp_in[sl]); // the staging buffers of this slot have left the host
-        ormask |= cpu_pack48(pool, a_host + off * ct_words, ctx->hst_a[sl], words);
-        ormask |= cpu_pack48(pool, b_host + off * ct_words, ctx->hst_b[sl], words);
+            cudaEventSynchronize(S.in); // the staging buffers of this slot have left the host
+        ormask |= cpu_pack48(pool, a_host + off * ct_words, S.hst_a, words);
+        ormask |= cpu_pack48(pool, b_host + off * ct_words, S.hst_b, words);
         if (ormask >> 48)
         {
             rc = fail(B200_E_INVALID, "ciphertext word does not fit the residue width of this level");
             break;
         }
         if (it >= NBUF)
-            cudaStreamWaitEvent(ctx->s_h2d, ctx->hp_out[sl], 0); // device slot free once its previous output left
-        cudaMemcpyAsync(ctx->dpk_a[sl], ctx->hst_a[sl], pbytes, cudaMemcpyHostToDevice, ctx->s_h2d);
-        cudaMemcpyAsync(ctx->dpk_b[sl], ctx->hst_b[sl], pbytes, cudaMemcpyHostToDevice, ctx->s_h2d);
-        cudaEventRecord(ctx->hp_in[sl], ctx->s_h2d);
-        cudaStreamWaitEvent(ctx->s_comp, ctx->hp_in[sl], 0);
-        B200_LAUNCH(unpack48_kernel, blocks_for((long long)groups, 256), 256, 0, ctx->s_comp, (const u64 *)ctx->dpk_a[sl], ctx->hp_a[sl],
+            cudaStreamWaitEvent(ctx->s_h2d, S.out, 0); // device slot free once its previous output left
+        cudaMemcpyAsync(S.dpk_a, S.hst_a, pbytes, cudaMemcpyHostToDevice, ctx->s_h2d);
+        cudaMemcpyAsync(S.dpk_b, S.hst_b, pbytes, cudaMemcpyHostToDevice, ctx->s_h2d);
+        cudaEventRecord(S.in, ctx->s_h2d);
+        cudaStreamWaitEvent(ctx->s_comp, S.in, 0);
+        B200_LAUNCH(unpack48_kernel, blocks_for((long long)groups, 256), 256, 0, ctx->s_comp, (const u64 *)S.dpk_a, S.a,
                     (long long)groups);
-        B200_LAUNCH(unpack48_kernel, blocks_for((long long)groups, 256), 256, 0, ctx->s_comp, (const u64 *)ctx->dpk_b[sl], ctx->hp_b[sl],
+        B200_LAUNCH(unpack48_kernel, blocks_for((long long)groups, 256), 256, 0, ctx->s_comp, (const u64 *)S.dpk_b, S.b,
                     (long long)groups);
         ctx->launches += 2;
-        rc = b200_multiply_relin(ctx, level, (const uint64_t *)ctx->hp_a[sl], (const uint64_t *)ctx->hp_b[sl],
-                                 (const uint64_t *)relin_key_dev, (uint64_t *)ctx->hp_o[sl], (uint64_t)cnt, ctx->s_comp);
-        B200_LAUNCH(pack48_kernel, blocks_for((long long)groups, 256), 256, 0, ctx->s_comp, (const u64 *)ctx->hp_o[sl], ctx->dpk_o[sl],
+        rc = b200_multiply_relin(ctx, level, (const uint64_t *)S.a, (const uint64_t *)S.b, (const uint64_t *)relin_key_dev,
+                                 (uint64_t *)S.o, (uint64_t)cnt, ctx->s_comp);
+        B200_LAUNCH(pack48_kernel, blocks_for((long long)groups, 256), 256, 0, ctx->s_comp, (const u64 *)S.o, S.dpk_o,
                     (long long)groups);
         ctx->launches++;
-        cudaEventRecord(ctx->hp_comp[sl], ctx->s_comp);
-        cudaStreamWaitEvent(ctx->s_d2h, ctx->hp_comp[sl], 0);
-        cudaMemcpyAsync(ctx->hst_o[sl], ctx->dpk_o[sl], pbytes, cudaMemcpyDeviceToHost, ctx->s_d2h);
-        cudaEventRecord(ctx->hp_out[sl], ctx->s_d2h);
+        cudaEventRecord(S.comp, ctx->s_comp);
+        cudaStreamWaitEvent(ctx->s_d2h, S.comp, 0);
+        cudaMemcpyAsync(S.hst_o, S.dpk_o, pbytes, cudaMemcpyDeviceToHost, ctx->s_d2h);
+        cudaEventRecord(S.out, ctx->s_d2h);
         if (it >= LAG)
             drain(it - LAG);
     }
-    cudaError_t e1 = cudaStreamSynchronize(ctx->s_h2d);
-    cudaError_t e2 = cudaStreamSynchronize(ctx->s_comp);
-    cudaError_t e3 = cudaStreamSynchronize(ctx->s_d2h);
-    if (rc)
+    if ((rc = finish_host_pipeline(ctx, rc)))
         return rc;
-    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
-        return fail(B200_E_CUDA, std::string("host pipeline: ") +
-                                     cudaGetErrorString(e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3)));
     for (int j = std::max(0, iters - LAG); j < iters; j++)
         drain(j);
     return 0;
@@ -4340,7 +4334,8 @@ int b200_multiply_relin_host(b200_ctx *ctx, int level, const uint64_t *a_host, c
     if (batch == 0)
         return 0;
     CU_TRY(cudaSetDevice(ctx->device));
-    std::lock_guard<std::mutex> lk(ctx->hp_mu);
+    StagingRing &R = ctx->ring;
+    std::lock_guard<std::mutex> lk(R.mu);
     const long long n = (long long)ctx->n;
     const int k = ctx->levels[level].k;
     const size_t ct_words = (size_t)2 * k * n;
@@ -4353,84 +4348,29 @@ int b200_multiply_relin_host(b200_ctx *ctx, int level, const uint64_t *a_host, c
     if (level_packs(ctx, level))
         return multiply_relin_host_packed(ctx, level, (const u64 *)a_host, (const u64 *)b_host, (const u64 *)relin_key_dev,
                                           (u64 *)out_host, batch, chunk, ct_words);
-    if ((rc = host_ring(ctx, (size_t)chunk * ct_words)))
+    if ((rc = R.reserve((size_t)chunk * ct_words)))
         return rc;
-    const int NBUF = b200_ctx::NBUF;
+    const int NBUF = StagingRing::NBUF;
     int it = 0;
     for (uint64_t off = 0; off < batch && rc == 0; off += (uint64_t)chunk, it++)
     {
-        const int sl = it % NBUF;
+        StagingRing::Slot &S = R.slot[it % NBUF];
         const long long cnt = (long long)std::min<uint64_t>((uint64_t)chunk, batch - off);
         const size_t bytes = (size_t)cnt * ct_words * sizeof(u64);
         if (it >= NBUF)
-            cudaStreamWaitEvent(ctx->s_h2d, ctx->hp_out[sl], 0); // slot free once its previous output left
-        cudaMemcpyAsync(ctx->hp_a[sl], a_host + off * ct_words, bytes, cudaMemcpyHostToDevice, ctx->s_h2d);
-        cudaMemcpyAsync(ctx->hp_b[sl], b_host + off * ct_words, bytes, cudaMemcpyHostToDevice, ctx->s_h2d);
-        cudaEventRecord(ctx->hp_in[sl], ctx->s_h2d);
-        cudaStreamWaitEvent(ctx->s_comp, ctx->hp_in[sl], 0);
-        rc = b200_multiply_relin(ctx, level, (const uint64_t *)ctx->hp_a[sl], (const uint64_t *)ctx->hp_b[sl], relin_key_dev,
-                                 (uint64_t *)ctx->hp_o[sl], (uint64_t)cnt, ctx->s_comp);
-        cudaEventRecord(ctx->hp_comp[sl], ctx->s_comp);
-        cudaStreamWaitEvent(ctx->s_d2h, ctx->hp_comp[sl], 0);
-        cudaMemcpyAsync(out_host + off * ct_words, ctx->hp_o[sl], bytes, cudaMemcpyDeviceToHost, ctx->s_d2h);
-        cudaEventRecord(ctx->hp_out[sl], ctx->s_d2h);
+            cudaStreamWaitEvent(ctx->s_h2d, S.out, 0); // slot free once its previous output left
+        cudaMemcpyAsync(S.a, a_host + off * ct_words, bytes, cudaMemcpyHostToDevice, ctx->s_h2d);
+        cudaMemcpyAsync(S.b, b_host + off * ct_words, bytes, cudaMemcpyHostToDevice, ctx->s_h2d);
+        cudaEventRecord(S.in, ctx->s_h2d);
+        cudaStreamWaitEvent(ctx->s_comp, S.in, 0);
+        rc = b200_multiply_relin(ctx, level, (const uint64_t *)S.a, (const uint64_t *)S.b, relin_key_dev, (uint64_t *)S.o,
+                                 (uint64_t)cnt, ctx->s_comp);
+        cudaEventRecord(S.comp, ctx->s_comp);
+        cudaStreamWaitEvent(ctx->s_d2h, S.comp, 0);
+        cudaMemcpyAsync(out_host + off * ct_words, S.o, bytes, cudaMemcpyDeviceToHost, ctx->s_d2h);
+        cudaEventRecord(S.out, ctx->s_d2h);
     }
-    cudaError_t e1 = cudaStreamSynchronize(ctx->s_h2d);
-    cudaError_t e2 = cudaStreamSynchronize(ctx->s_comp);
-    cudaError_t e3 = cudaStreamSynchronize(ctx->s_d2h);
-    if (rc)
-        return rc;
-    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
-        return fail(B200_E_CUDA, std::string("host pipeline: ") +
-                                     cudaGetErrorString(e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3)));
-    return 0;
-}
-
-int b200_ntt_roundtrip_host(b200_ctx *ctx, int level, const uint64_t *in_host, uint64_t *out_host, uint64_t items)
-{
-    int rc = check_level(ctx, level);
-    if (rc)
-        return rc;
-    if (!in_host || !out_host)
-        return fail(B200_E_NULL, "null pointer");
-    if (items == 0)
-        return 0;
-    CU_TRY(cudaSetDevice(ctx->device));
-    std::lock_guard<std::mutex> lk(ctx->hp_mu);
-    const size_t words = (size_t)ctx->levels[level].k * ctx->n;
-    long long chunk = 512;
-    if ((uint64_t)chunk > items)
-        chunk = (long long)items;
-    if ((rc = host_ring(ctx, (size_t)chunk * words)))
-        return rc;
-    const int NBUF = b200_ctx::NBUF;
-    int it = 0;
-    for (uint64_t off = 0; off < items && rc == 0; off += (uint64_t)chunk, it++)
-    {
-        const int sl = it % NBUF;
-        const long long cnt = (long long)std::min<uint64_t>((uint64_t)chunk, items - off);
-        const size_t bytes = (size_t)cnt * words * sizeof(u64);
-        if (it >= NBUF)
-            cudaStreamWaitEvent(ctx->s_h2d, ctx->hp_out[sl], 0);
-        cudaMemcpyAsync(ctx->hp_a[sl], in_host + off * words, bytes, cudaMemcpyHostToDevice, ctx->s_h2d);
-        cudaEventRecord(ctx->hp_in[sl], ctx->s_h2d);
-        cudaStreamWaitEvent(ctx->s_comp, ctx->hp_in[sl], 0);
-        rc = b200_ntt_forward(ctx, level, (uint64_t *)ctx->hp_a[sl], (uint64_t)cnt, ctx->s_comp);
-        if (!rc)
-            rc = b200_ntt_inverse(ctx, level, (uint64_t *)ctx->hp_a[sl], (uint64_t)cnt, ctx->s_comp);
-        cudaEventRecord(ctx->hp_comp[sl], ctx->s_comp);
-        cudaStreamWaitEvent(ctx->s_d2h, ctx->hp_comp[sl], 0);
-        cudaMemcpyAsync(out_host + off * words, ctx->hp_a[sl], bytes, cudaMemcpyDeviceToHost, ctx->s_d2h);
-        cudaEventRecord(ctx->hp_out[sl], ctx->s_d2h);
-    }
-    cudaError_t e1 = cudaStreamSynchronize(ctx->s_h2d);
-    cudaError_t e2 = cudaStreamSynchronize(ctx->s_comp);
-    cudaError_t e3 = cudaStreamSynchronize(ctx->s_d2h);
-    if (rc)
-        return rc;
-    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess)
-        return fail(B200_E_CUDA, "host pipeline failed");
-    return 0;
+    return finish_host_pipeline(ctx, rc);
 }
 
 } // extern "C"

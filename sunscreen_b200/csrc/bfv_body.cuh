@@ -31,24 +31,10 @@ struct LevelDev
     int k, nB, nBsk;
     const PrimeDev *q;   // [k]
     const PrimeDev *bsk; // [nBsk] (B..., m_sk)
-    u64 m_sk, t;
+    u64 t;
     PrimeDev t_mod;
     PrimeDev gamma;
-    // lift
-    const u64 *lift_c;   // [2k] shoup pairs
-    const u64 *lift_mat; // [nBsk*k]
-    const u64 *lift_mt;  // [k]
-    const u64 *lift_qm;  // [nBsk]
-    u64 neg_inv_q_mod_mt;
-    // scale
-    const u64 *scale_c;    // [2k]
-    const u64 *scale_tq;   // [nBsk]
-    const u64 *scale_mat;  // [nBsk*k]
-    const u64 *sk_c;       // [2nB]
-    const u64 *sk_mat_q;   // [k*nB]
-    const u64 *sk_mat_msk; // [nB]
-    const u64 *sk_prod_b_q;// [k]
-    u64 sk_inv_b_msk;
+    // (the BEHZ lift and scale constants travel as kernel PARAMETERS: LiftIntC / ScaleIntC, LiftFpC / ScaleFpC below)
     // last-prime division (mod switch at this level)
     const u64 *inv_qlast;  // [2(k-1)]
     // plaintext
@@ -61,7 +47,6 @@ struct LevelDev
     int fp;
     const double *dq;        // [2k]     {q_i, 1/q_i}
     const double *dbsk;      // [2nBsk]  {p_j, 1/p_j}
-    // (the BEHZ base-conversion constants of the FP64 path travel as kernel PARAMETERS: LiftFpC / ScaleFpC below)
     // decrypt
     const u64 *dec_c;      // [2k]
     const u64 *dec_mat_t;  // [k]

@@ -90,7 +90,6 @@ _SIGS = {
     "b200_any_nonzero": [vp, C.c_int, vp, C.c_int, vp, u64, vp],
     "b200_expand_signed": [vp, C.c_int, vp, C.c_int, vp, vp],
     "b200_multiply_relin_host": [vp, C.c_int, vp, vp, vp, vp, u64],
-    "b200_ntt_roundtrip_host": [vp, C.c_int, vp, vp, u64],
 }
 
 EXPORTS = sorted(list(_SIGS) + ["b200_last_error", "b200_device_count", "b200_ctx_destroy", "b200_launch_count"])
@@ -352,6 +351,3 @@ class B200Context:
     def multiply_relin_host(self, a_host, b_host, rlk_dev, out_host, batch, level=None):
         self.L.call("b200_multiply_relin_host", self.h, self._lv(level), vp(ptr(a_host)), vp(ptr(b_host)), vp(ptr(rlk_dev)),
                     vp(ptr(out_host)), u64(batch))
-
-    def ntt_roundtrip_host(self, in_host, out_host, items, level=None):
-        self.L.call("b200_ntt_roundtrip_host", self.h, self._lv(level), vp(ptr(in_host)), vp(ptr(out_host)), u64(items))

@@ -6,6 +6,8 @@
 // loops, see ntt_body.cuh).  Nothing here is compiled into sunscreen_b200/libb200bfv.so.
 #pragma once
 #include <algorithm>
+#include <atomic>
+#include <cstdint>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
@@ -30,6 +32,37 @@ struct dim3 { unsigned x, y, z; dim3(unsigned a = 1, unsigned b = 1, unsigned c 
 static thread_local dim3 threadIdx, blockIdx, blockDim, gridDim;
 static thread_local void *emu_shared = nullptr;
 
+// Resource accounting for tests/test_context_lifetime.py.  Streams, events and memory pools are distinct non-null handles;
+// emu_live counts them together with every cudaMalloc, cudaMallocHost and pool allocation not yet released.  A budget
+// n >= 0 lets n more of these creations succeed and fails every later one, as an exhausted device would (-1: no limit).
+static std::atomic<long long> emu_live{ 0 }, emu_budget{ -1 };
+static std::atomic<uintptr_t> emu_next_handle{ 0 };
+extern "C" long long b200_emu_live_resources(void) { return emu_live; }
+extern "C" void b200_emu_alloc_budget(long long n) { emu_budget = n; }
+inline bool emu_acquire()
+{
+    if (emu_budget == 0)
+        return false;
+    if (emu_budget > 0)
+        emu_budget--;
+    emu_live++;
+    return true;
+}
+inline cudaError_t emu_create(void **h)
+{
+    if (!emu_acquire())
+        return 2;
+    *h = (void *)(++emu_next_handle * 16);
+    return 0;
+}
+inline cudaError_t emu_destroy(void *h)
+{
+    if (!h)
+        return 1; // the runtime rejects a null handle
+    emu_live--;
+    return 0;
+}
+
 inline cudaError_t cudaGetDeviceCount(int *c) { *c = 1; return 0; }
 inline cudaError_t cudaSetDevice(int) { return 0; }
 inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { *p = cudaDeviceProp(); return 0; }
@@ -38,12 +71,24 @@ inline cudaError_t cudaDeviceGetDefaultMemPool(cudaMemPool_t *p, int) { *p = nul
 inline cudaError_t cudaMemPoolSetAttribute(cudaMemPool_t, int, void *) { return 0; }
 enum { cudaMemAllocationTypePinned = 1, cudaMemHandleTypeNone = 0, cudaMemLocationTypeDevice = 1 };
 struct cudaMemPoolProps { int allocType, handleTypes; struct { int type, id; } location; };
-inline cudaError_t cudaMemPoolCreate(cudaMemPool_t *p, const cudaMemPoolProps *) { *p = nullptr; return 0; }
-inline cudaError_t cudaMemPoolDestroy(cudaMemPool_t) { return 0; }
+inline cudaError_t cudaMemPoolCreate(cudaMemPool_t *p, const cudaMemPoolProps *) { return emu_create(p); }
+inline cudaError_t cudaMemPoolDestroy(cudaMemPool_t p) { return emu_destroy(p); }
 inline cudaError_t cudaDeviceSynchronize() { return 0; }
 inline cudaError_t cudaGetLastError() { return 0; }
-inline cudaError_t cudaMalloc(void **p, size_t b) { *p = std::malloc(b ? b : 8); return *p ? 0 : 2; }
-inline cudaError_t cudaFree(void *p) { std::free(p); return 0; }
+inline cudaError_t cudaMalloc(void **p, size_t b)
+{
+    if (!emu_acquire())
+        return 2;
+    *p = std::malloc(b ? b : 8);
+    return *p ? 0 : 2;
+}
+inline cudaError_t cudaFree(void *p)
+{
+    if (p)
+        emu_live--;
+    std::free(p);
+    return 0;
+}
 inline cudaError_t cudaMallocHost(void **p, size_t b) { return cudaMalloc(p, b); }
 inline cudaError_t cudaFreeHost(void *p) { return cudaFree(p); }
 inline cudaError_t cudaMallocAsync(void **p, size_t b, cudaStream_t) { return cudaMalloc(p, b); }
@@ -52,13 +97,13 @@ inline cudaError_t cudaFreeAsync(void *p, cudaStream_t) { return cudaFree(p); }
 inline cudaError_t cudaMemcpy(void *d, const void *s, size_t b, cudaMemcpyKind) { std::memmove(d, s, b); return 0; }
 inline cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t b, cudaMemcpyKind, cudaStream_t) { std::memmove(d, s, b); return 0; }
 inline cudaError_t cudaMemsetAsync(void *d, int v, size_t b, cudaStream_t) { std::memset(d, v, b); return 0; }
-inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, int) { *s = nullptr; return 0; }
-inline cudaError_t cudaStreamDestroy(cudaStream_t) { return 0; }
+inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, int) { return emu_create(s); }
+inline cudaError_t cudaStreamDestroy(cudaStream_t s) { return emu_destroy(s); }
 inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return 0; }
 inline cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, int) { return 0; }
-inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t *e, int) { *e = nullptr; return 0; }
+inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t *e, int) { return emu_create(e); }
 inline cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t) { return 0; }
-inline cudaError_t cudaEventDestroy(cudaEvent_t) { return 0; }
+inline cudaError_t cudaEventDestroy(cudaEvent_t e) { return emu_destroy(e); }
 inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return 0; }
 inline unsigned long long __ldg(const unsigned long long *p) { return *p; }
 inline double __ldg(const double *p) { return *p; }
