@@ -107,6 +107,22 @@ int b200_ntt_inverse(b200_ctx *ctx, int level, uint64_t *data, uint64_t items, v
 /* negacyclic NTT modulo the plain modulus t over [items][n] (BatchEncoder encode = inverse, decode = forward) */
 int b200_plain_ntt(b200_ctx *ctx, uint64_t *data, uint64_t items, int inverse, void *stream);
 
+/* ---- slots in and out (BatchEncoder, S/batchencoder.cpp), batched; B200_E_INVALID when the parameters do not batch ---- */
+/* values: device [items][count] (count <= n; NULL allowed when count == 0), read as int64_t when is_signed -> plain_out:
+   device [items][n] coefficients mod t, the words of BatchEncoder_Encode1 (unsigned: each value reduced mod t) or
+   BatchEncoder_Encode2 (signed: a negative x becomes t + x); slots at and beyond count are zero.  Multiply-ready operands:
+   follow with b200_plain_to_ntt. */
+int b200_batch_encode(b200_ctx *ctx, const uint64_t *values, uint64_t count, int is_signed, uint64_t *plain_out, uint64_t items,
+                      void *stream);
+/* plain: device [items][n] coefficient form (zero-padded, not modified) -> slots_out: device [items][n], uint64_t mod t
+   (BatchEncoder_Decode1) or, with is_signed, int64_t centred v > t/2 ? v - t : v (BatchEncoder_Decode2) */
+int b200_batch_decode(b200_ctx *ctx, const uint64_t *plain, int is_signed, uint64_t *slots_out, uint64_t items, void *stream);
+/* b200_decrypt followed by b200_batch_decode, and with norm_out != NULL also b200_noise_norm, from one secret-key phase per
+   call: slots_out device [batch][n]; norm_out HOST [batch][words] as b200_noise_norm fills it (the call then returns after
+   completion; with norm_out == NULL it is asynchronous and `words` is not read) */
+int b200_decrypt_slots(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, int is_signed,
+                       uint64_t *slots_out, uint64_t *norm_out, int words, uint64_t batch, void *stream);
+
 /* ---- ciphertext arithmetic, batched over `batch` independent items (device pointers) ---- */
 int b200_add(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, uint64_t *out, int size, uint64_t batch,
              void *stream);

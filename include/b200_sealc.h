@@ -195,7 +195,7 @@ SEAL_C_FUNC Encryptor_EncryptSymmetricReturnComponentsSetSeed(void *thisptr, voi
                                                               void *e_destination, void *remainder_destination, void *seed,
                                                               void *pool_handle);
 
-/* ---- BatchEncoder (S/c/batchencoder.h): slot permutation on the host, negacyclic NTT mod t on the GPU ---- */
+/* ---- BatchEncoder (S/c/batchencoder.h): slot permutation and negacyclic NTT mod t on the GPU ---- */
 SEAL_C_FUNC BatchEncoder_Create(void *context, void **batch_encoder);
 SEAL_C_FUNC BatchEncoder_Destroy(void *thisptr);
 SEAL_C_FUNC BatchEncoder_Encode1(void *thisptr, uint64_t count, uint64_t *values, void *destination);
@@ -324,6 +324,21 @@ SEAL_C_FUNC B200_Evaluator_RotateRowsStepsBatch(void *thisptr, uint64_t count, v
    baby or giant 0 and a call where every term is absent are E_INVALIDARG.  Destinations may alias encrypteds. */
 SEAL_C_FUNC B200_Evaluator_LinearTransform(void *thisptr, uint64_t count, void **encrypteds, uint64_t baby, uint64_t giant, void **plains,
                                            void *galois_keys, void **destinations);
+
+/* slots in and out for many plaintexts / ciphertexts at once, one transfer each way and one launch sequence per call:
+   EncodeBatch: destinations[i] receives the plaintext BatchEncoder_Encode1 (is_signed: Encode2, the words read as int64_t)
+   gives for row i of `values`, one host buffer [count][values_per_item].  Same checks and HRESULTs as those calls.
+   DecodeBatch: slots_out (host [count][n], uint64_t or with is_signed int64_t) receives BatchEncoder_Decode1/2 of plains[i].
+   Same checks and HRESULTs as those calls, all made before any work.
+   DecryptSlotsBatch: slots_out (host [count][n]) receives BatchEncoder_Decode1/2(Decryptor_Decrypt(encrypteds[i])) and, when
+   budgets != NULL, budgets[i] Decryptor_InvariantNoiseBudget(encrypteds[i]), from one secret-key phase per item.  Same checks
+   and HRESULTs as those calls, all made before any work, except: all encrypteds must have one size and one level
+   (E_INVALIDARG).  A decryptor and an encoder of different contexts are E_INVALIDARG. */
+SEAL_C_FUNC B200_BatchEncoder_EncodeBatch(void *encoder, uint64_t count, uint64_t values_per_item, const uint64_t *values,
+                                          bool is_signed, void **destinations);
+SEAL_C_FUNC B200_BatchEncoder_DecodeBatch(void *encoder, uint64_t count, void **plains, bool is_signed, void *slots_out);
+SEAL_C_FUNC B200_Decryptor_DecryptSlotsBatch(void *decryptor, void *encoder, uint64_t count, void **encrypteds, bool is_signed,
+                                             void *slots_out, int *budgets);
 
 /* ---- debug aids (tests only; not part of the seal_fhe surface) ---- */
 /* `count` (1 ... 64) per-handle calls of one kind run as if they had arrived together at the combiner: kind 0

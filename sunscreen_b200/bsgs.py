@@ -1,4 +1,5 @@
-"""Slot vectors of a baby-step giant-step (BSGS) slot-wise linear transform, for B200Context.linear_transform.
+"""Slot vectors of a baby-step giant-step (BSGS) slot-wise linear transform, and their NTT-form plaintexts, for
+B200Context.linear_transform.
 
 With batching, a ciphertext holds a 2 x n/2 matrix of slots, and rotate_rows(s) rotates both rows left by s.  A d x d matrix M
 (d divides n/2) applied to a vector v replicated with period d along a row is the diagonal method
@@ -67,3 +68,13 @@ def apply_slotwise(mats, v, n, t):
         y = m.dot(x) % t
         out[r * h:(r + 1) * h] = np.array([int(y[i % d]) for i in range(h)], dtype=np.uint64)
     return out
+
+
+def bsgs_plain_ntt(ctx, vecs, coeffs, out, level=None, stream=None):
+    """The transform's plain_ntt operand prepared on the device: the slot vectors `vecs` [giant][baby][n] (device, from
+    bsgs_plain_vectors) batch-encoded into `coeffs` [giant * baby][n] (device scratch), then lifted to NTT form into `out`
+    [giant][baby][k][n] with the multiply rule.  Two calls whatever the number of terms."""
+    from sunscreen_b200.lib import PLAIN_NTT_MULTIPLY
+    items = int(vecs.shape[0]) * int(vecs.shape[1])
+    ctx.batch_encode(vecs, ctx.n, coeffs, items, stream=stream)
+    ctx.plain_to_ntt(coeffs, items, out, rule=PLAIN_NTT_MULTIPLY, level=level, stream=stream)

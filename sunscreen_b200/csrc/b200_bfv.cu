@@ -1212,6 +1212,37 @@ __global__ void fill_u32_kernel(u32 *p, u32 v, long long total)
         p[idx] = v;
 }
 
+// BatchEncoder::encode before its inverse transform (S/batchencoder.cpp:110-193): value i of each item, reduced mod t
+// (signed: a negative x is first lifted to t + x), goes to coefficient map[i]; slots at and beyond `count` get zero.  The map
+// is a permutation, so every word of `plain` is written.
+__global__ void slot_scatter_kernel(const u32 *map, u64 t, const u64 *vals, long long count, int is_signed, u64 *plain, int logn,
+                                    long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long i = idx & ((1LL << logn) - 1), item = idx >> logn;
+    u64 v = 0;
+    if (i < count)
+    {
+        const u64 x = vals[item * count + i];
+        v = (is_signed && (long long)x < 0 ? t + x : x) % t;
+    }
+    plain[(item << logn) + map[i]] = v;
+}
+
+// BatchEncoder::decode after its forward transform (S/batchencoder.cpp:278-360): slot i of each item is coefficient map[i];
+// signed, a value above t/2 becomes value - t (two's complement)
+__global__ void slot_gather_kernel(const u32 *map, u64 t, const u64 *plain, int is_signed, u64 *slots, int logn, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long i = idx & ((1LL << logn) - 1), item = idx >> logn;
+    const u64 v = plain[(item << logn) + map[i]];
+    slots[idx] = is_signed && v > (t >> 1) ? v - t : v;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------------------
@@ -1414,6 +1445,7 @@ struct b200_ctx
     std::vector<FpMasks> fp_masks; // per device prime (FP64 path): renorm masks per schedule (b200_debug_fp_masks)
     std::vector<u64> prime_value;  // per device prime
     int plain_prime_idx = -1;    // index of the plain modulus in the device prime tables (-1: no batching)
+    const u32 *d_slot_map = nullptr; // [n] BatchEncoder slot -> coefficient index (batching only)
     PrimeDev *d_primes = nullptr;       // [all primes] key primes first
     std::vector<LevelDev> levels;       // device pointers inside
     const u64 *d_inv_qsp = nullptr;     // key level's inv_qlast: q_sp^-1 mod q_i
@@ -1510,6 +1542,9 @@ static int build_device(b200_ctx *ctx)
     {
         ctx->plain_prime_idx = (int)allp.size();
         allp.push_back(&H.plain_ntt);
+        u32 *map = nullptr;
+        UP(H.slot_index_map, &map);
+        ctx->d_slot_map = map;
     }
     std::vector<NttPrime> np(allp.size());
     std::vector<PrimeDev> pd(allp.size());
@@ -3020,6 +3055,77 @@ int b200_plain_ntt(b200_ctx *ctx, uint64_t *data, uint64_t items, int inverse, v
     return launch_ntt<true>(ctx, jd, (u64 *)data, stride, (u64 *)data, stride, (long long)items, 0, (cudaStream_t)stream);
 }
 
+// ---- slots in and out (BatchEncoder) ----
+static int check_batching(b200_ctx *ctx)
+{
+    if (ctx->plain_prime_idx < 0)
+        return fail(B200_E_INVALID, "encryption parameters are not valid for batching");
+    return 0;
+}
+
+// slots [items][n] of the coefficient-form plaintexts `plain`: the forward transform mod t from `plain` into `work` (which may
+// be `plain`), then the gather through the slot map
+static int slots_from_plain(b200_ctx *ctx, const u64 *plain, u64 *work, int is_signed, u64 *slots_out, long long items,
+                            cudaStream_t s)
+{
+    JobDesc jd;
+    int rc = dense_job(ctx, "plain", std::vector<int>(1, ctx->plain_prime_idx), &jd);
+    if (rc)
+        return rc;
+    const long long n = (long long)ctx->n, total = items * n;
+    if ((rc = launch_ntt<true>(ctx, jd, plain, n, work, n, items, 0, s)))
+        return rc;
+    B200_LAUNCH(slot_gather_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_slot_map, ctx->host->t, (const u64 *)work, is_signed,
+                slots_out, ctx->logn, total);
+    ctx->launches++;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+int b200_batch_encode(b200_ctx *ctx, const uint64_t *values, uint64_t count, int is_signed, uint64_t *plain_out, uint64_t items,
+                      void *stream)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if ((!values && count) || !plain_out)
+        return fail(B200_E_NULL, "null pointer");
+    int rc = check_batching(ctx);
+    if (rc)
+        return rc;
+    if (count > ctx->n)
+        return fail(B200_E_INVALID, "values_matrix size is too large");
+    if (items == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    const long long total = (long long)items * (long long)ctx->n;
+    cudaStream_t s = (cudaStream_t)stream;
+    B200_LAUNCH(slot_scatter_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_slot_map, ctx->host->t, (const u64 *)values,
+                (long long)count, is_signed, (u64 *)plain_out, ctx->logn, total);
+    ctx->launches++;
+    CU_TRY(cudaGetLastError());
+    return b200_plain_ntt(ctx, plain_out, items, 1, stream);
+}
+
+int b200_batch_decode(b200_ctx *ctx, const uint64_t *plain, int is_signed, uint64_t *slots_out, uint64_t items, void *stream)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if (!plain || !slots_out)
+        return fail(B200_E_NULL, "null pointer");
+    int rc = check_batching(ctx);
+    if (rc)
+        return rc;
+    if (items == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    u64 *work = nullptr;
+    if ((rc = scr.get((size_t)items * ctx->n, &work)))
+        return rc;
+    return slots_from_plain(ctx, (const u64 *)plain, work, is_signed, (u64 *)slots_out, (long long)items, s);
+}
+
 // ---- add / sub / negate ----
 static int addsub(b200_ctx *ctx, int level, const u64 *a, const u64 *b, u64 *out, int size, uint64_t batch, void *stream,
                   int mode)
@@ -3916,6 +4022,18 @@ static int sk_phase(b200_ctx *ctx, int level, const u64 *ct, int size, const u64
     return launch_ntt<false>(ctx, jd, acc, (long long)k * n, acc, (long long)k * n, batch, 0, s);
 }
 
+// plaintext coefficients [batch][n] from the phase without c0 (sk_phase), which serves as scratch
+static int decrypt_from_phase(b200_ctx *ctx, int level, const u64 *ct, int size, u64 *acc, u64 *plain_out, long long batch,
+                              cudaStream_t s)
+{
+    const long long n = (long long)ctx->n, total = batch * n;
+    const LevelDev &L = ctx->levels[level];
+    DISPATCH_K(L.k, B200_LAUNCH(decrypt_kernel<KK>, blocks_for(total, EB), EB, 0, s, L, size, ct, acc, plain_out, n, total));
+    ctx->launches++;
+    CU_TRY(cudaGetLastError());
+    return 0;
+}
+
 int b200_decrypt(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, uint64_t *plain_out,
                  uint64_t batch, void *stream)
 {
@@ -3925,24 +4043,14 @@ int b200_decrypt(b200_ctx *ctx, int level, const uint64_t *ct, int size, const u
     if (batch == 0)
         return 0;
     CU_TRY(cudaSetDevice(ctx->device));
-    const long long n = (long long)ctx->n;
-    const LevelDev &L = ctx->levels[level];
-    const int k = L.k;
     cudaStream_t s = (cudaStream_t)stream;
     Scratch scr(ctx, s);
     u64 *acc = nullptr;
-    if ((rc = scr.get((size_t)batch * k * n, &acc)))
+    if ((rc = scr.get((size_t)batch * ctx->levels[level].k * ctx->n, &acc)))
         return rc;
     if ((rc = sk_phase(ctx, level, (const u64 *)ct, size, (const u64 *)sk_powers_ntt, acc, (long long)batch, scr, s)))
         return rc;
-    {
-        const long long total = (long long)batch * n;
-        DISPATCH_K(k, B200_LAUNCH(decrypt_kernel<KK>, blocks_for(total, EB), EB, 0, s, L, size, (const u64 *)ct, acc,
-                                                                              (u64 *)plain_out, n, total));
-        ctx->launches++;
-    }
-    CU_TRY(cudaGetLastError());
-    return 0;
+    return decrypt_from_phase(ctx, level, (const u64 *)ct, size, acc, (u64 *)plain_out, (long long)batch, s);
 }
 
 // phase = c0 + sum_{j>=1} c_j * s^j  (coefficient form, canonical), [batch][k][n]
@@ -3972,17 +4080,13 @@ int b200_ct_sk_phase(b200_ctx *ctx, int level, const uint64_t *ct, int size, con
     return 0;
 }
 
-// infinity norm of the centred t * (c0 + sum_j c_j s^j) mod Q of each item as a little-endian multi-precision integer
-// (Decryptor::invariant_noise_internal, S/decryptor.cpp:424-485).  norm_out: HOST array [batch][words]; the call returns
-// after the result has arrived.
-int b200_noise_norm(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, uint64_t *norm_out,
-                    int words, uint64_t batch, void *stream)
+// ---- infinity norm of the centred t * (c0 + sum_j c_j s^j) mod Q of each item (Decryptor::invariant_noise_internal,
+// S/decryptor.cpp:424-485), in three steps: the level's constants, the block maxima of the phase, and their merge on the host ----
+
+// the constants of noise_norm_kernel at `level` (built on first use and kept with the context) and W, the words of Q; refuses
+// a norm_out of fewer than W + 1 words
+static int noise_setup(b200_ctx *ctx, int level, int words, u64 **consts_out, int *W_out)
 {
-    int rc = check_sk_args(ctx, level, ct, size, sk_powers_ntt, norm_out);
-    if (rc)
-        return rc;
-    CU_TRY(cudaSetDevice(ctx->device));
-    const long long n = (long long)ctx->n;
     const LevelHost &Lh = ctx->host->levels[level];
     const int k = ctx->levels[level].k;
     u64 *consts = nullptr;
@@ -4027,6 +4131,7 @@ int b200_noise_norm(b200_ctx *ctx, int level, const uint64_t *ct, int size, cons
                 for (int i = 0; i <= W; i++)
                     half[i] = (tmp[i] >> 1) | (i < W ? tmp[i + 1] << 63 : 0);
             }
+            int rc;
             if ((rc = upload(ctx, h, &consts)))
                 return rc;
             ctx->noise_consts[level] = std::make_pair(consts, W);
@@ -4039,28 +4144,34 @@ int b200_noise_norm(b200_ctx *ctx, int level, const uint64_t *ct, int size, cons
     }
     if (words < W + 1)
         return fail(B200_E_INVALID, "norm_out holds fewer words than the coefficient modulus");
-    for (size_t i = 0; i < (size_t)batch * words; i++)
-        norm_out[i] = 0;
-    if (batch == 0)
-        return 0;
-    cudaStream_t s = (cudaStream_t)stream;
-    Scratch scr(ctx, s);
-    u64 *acc = nullptr, *bm = nullptr;
-    const int NT = 128, CHUNK = 128, WW = W + 1;
-    const int blocks = (int)((n + CHUNK - 1) / CHUNK);
-    if ((rc = scr.get((size_t)batch * k * n, &acc)))
+    *consts_out = consts;
+    *W_out = W;
+    return 0;
+}
+
+static const int NOISE_NT = 128, NOISE_CHUNK = 128;
+
+// block maxima [batch][blocks][W + 1] of the centred t * (c0 + dot) into *bm (scratch); `dot` is the phase without c0 (sk_phase)
+static int noise_blocks(b200_ctx *ctx, int level, const u64 *consts, int W, const u64 *ct, int size, const u64 *dot, long long batch,
+                        Scratch &scr, cudaStream_t s, u64 **bm)
+{
+    const long long n = (long long)ctx->n;
+    const int blocks = (int)((n + NOISE_CHUNK - 1) / NOISE_CHUNK), WW = W + 1;
+    int rc;
+    if ((rc = scr.get((size_t)batch * blocks * WW, bm)))
         return rc;
-    if ((rc = scr.get((size_t)batch * blocks * WW, &bm)))
-        return rc;
-    if ((rc = sk_phase(ctx, level, (const u64 *)ct, size, (const u64 *)sk_powers_ntt, acc, (long long)batch, scr, s)))
-        return rc;
-    {
-        dim3 grid((unsigned)blocks, (unsigned)batch);
-        B200_LAUNCH(noise_norm_kernel, grid, NT, (size_t)NT * WW * 8, s, (const u64 *)consts, k, W, size, (const u64 *)ct,
-                    (const u64 *)acc, n, CHUNK, bm);
-        ctx->launches++;
-    }
+    dim3 grid((unsigned)blocks, (unsigned)batch);
+    B200_LAUNCH(noise_norm_kernel, grid, NOISE_NT, (size_t)NOISE_NT * WW * 8, s, consts, ctx->levels[level].k, W, size, ct, dot, n,
+                NOISE_CHUNK, *bm);
+    ctx->launches++;
     CU_TRY(cudaGetLastError());
+    return 0;
+}
+
+// waits for `s`, then merges the block maxima of noise_blocks into norm_out (HOST [batch][words], zeroed by the caller)
+static int noise_merge(b200_ctx *ctx, int W, const u64 *bm, uint64_t *norm_out, int words, uint64_t batch, cudaStream_t s)
+{
+    const int blocks = (int)((ctx->n + NOISE_CHUNK - 1) / NOISE_CHUNK), WW = W + 1;
     std::vector<u64> hb((size_t)batch * blocks * WW);
     CU_TRY(cudaMemcpyAsync(hb.data(), bm, hb.size() * 8, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaStreamSynchronize(s));
@@ -4075,6 +4186,74 @@ int b200_noise_norm(b200_ctx *ctx, int level, const uint64_t *ct, int size, cons
         }
     }
     return 0;
+}
+
+// norm_out: HOST array [batch][words]; the call returns after the result has arrived.
+int b200_noise_norm(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, uint64_t *norm_out,
+                    int words, uint64_t batch, void *stream)
+{
+    int rc = check_sk_args(ctx, level, ct, size, sk_powers_ntt, norm_out);
+    if (rc)
+        return rc;
+    CU_TRY(cudaSetDevice(ctx->device));
+    u64 *consts = nullptr;
+    int W = 0;
+    if ((rc = noise_setup(ctx, level, words, &consts, &W)))
+        return rc;
+    for (size_t i = 0; i < (size_t)batch * words; i++)
+        norm_out[i] = 0;
+    if (batch == 0)
+        return 0;
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    u64 *acc = nullptr, *bm = nullptr;
+    if ((rc = scr.get((size_t)batch * ctx->levels[level].k * ctx->n, &acc)))
+        return rc;
+    if ((rc = sk_phase(ctx, level, (const u64 *)ct, size, (const u64 *)sk_powers_ntt, acc, (long long)batch, scr, s)))
+        return rc;
+    if ((rc = noise_blocks(ctx, level, consts, W, (const u64 *)ct, size, acc, (long long)batch, scr, s, &bm)))
+        return rc;
+    return noise_merge(ctx, W, bm, norm_out, words, batch, s);
+}
+
+// decrypt, decode and (norm_out != NULL) noise norm from one secret-key phase: the phase's block maxima are taken before
+// decrypt_kernel adds c0 into it, the plaintext goes to scratch, and the slots are decoded from there
+int b200_decrypt_slots(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, int is_signed,
+                       uint64_t *slots_out, uint64_t *norm_out, int words, uint64_t batch, void *stream)
+{
+    int rc = check_sk_args(ctx, level, ct, size, sk_powers_ntt, slots_out);
+    if (rc)
+        return rc;
+    if ((rc = check_batching(ctx)))
+        return rc;
+    CU_TRY(cudaSetDevice(ctx->device));
+    u64 *consts = nullptr;
+    int W = 0;
+    if (norm_out)
+    {
+        if ((rc = noise_setup(ctx, level, words, &consts, &W)))
+            return rc;
+        for (size_t i = 0; i < (size_t)batch * words; i++)
+            norm_out[i] = 0;
+    }
+    if (batch == 0)
+        return 0;
+    const long long n = (long long)ctx->n;
+    const int k = ctx->levels[level].k;
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    u64 *acc = nullptr, *plain = nullptr, *bm = nullptr;
+    if ((rc = scr.get((size_t)batch * k * n, &acc)) || (rc = scr.get((size_t)batch * n, &plain)))
+        return rc;
+    if ((rc = sk_phase(ctx, level, (const u64 *)ct, size, (const u64 *)sk_powers_ntt, acc, (long long)batch, scr, s)))
+        return rc;
+    if (norm_out && (rc = noise_blocks(ctx, level, consts, W, (const u64 *)ct, size, acc, (long long)batch, scr, s, &bm)))
+        return rc;
+    if ((rc = decrypt_from_phase(ctx, level, (const u64 *)ct, size, acc, plain, (long long)batch, s)))
+        return rc;
+    if ((rc = slots_from_plain(ctx, plain, plain, is_signed, (u64 *)slots_out, (long long)batch, s)))
+        return rc;
+    return norm_out ? noise_merge(ctx, W, bm, norm_out, words, batch, s) : 0;
 }
 
 int b200_is_transparent(b200_ctx *ctx, int level, const uint64_t *ct, int size, uint32_t *flags_out, uint64_t batch,

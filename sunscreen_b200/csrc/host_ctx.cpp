@@ -440,6 +440,17 @@ BfvHostContext::BfvHostContext(size_t poly_modulus_degree, const std::vector<u64
     {
         plain_ntt = make_ntt_prime(t, logn);
         using_batching = true;
+        // BatchEncoder::populate_matrix_reps_index_map (S/batchencoder.cpp:64-88): slot i of the 2 x n/2 matrix lives at
+        // coefficient slot_index_map[i] of the transformed polynomial
+        const size_t row = n >> 1, m = n << 1;
+        slot_index_map.resize(n);
+        u64 pos = 1;
+        for (size_t i = 0; i < row; i++)
+        {
+            slot_index_map[i] = (uint32_t)reverse_bits((pos - 1) >> 1, logn);
+            slot_index_map[row | i] = (uint32_t)reverse_bits((m - pos - 1) >> 1, logn);
+            pos = (pos * 3) & (m - 1);
+        }
     }
 
     // Auxiliary BEHZ base: m_sk, gamma, then B.

@@ -137,6 +137,7 @@ struct BfvHostContext
     bool using_keyswitching = false;  // K > 1
     bool using_batching = false;      // t prime and t == 1 mod 2n
     NttPrimeHost plain_ntt;           // tables mod t when using_batching (for BatchEncoder)
+    std::vector<uint32_t> slot_index_map; // [n] when using_batching: coefficient index of each slot (BatchEncoder)
 
     // Build everything. Throws std::invalid_argument for parameters the reference would reject
     // (non-power-of-two n, moduli not == 1 mod 2n, duplicates, t >= q_i is allowed, ...).

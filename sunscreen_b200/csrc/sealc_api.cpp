@@ -2856,6 +2856,18 @@ static void noise_norm(Decryptor_ *d, Ciphertext_ &ct, std::vector<u64> &norm_ou
         q_bits_out = Q.bit_length();
     }
 }
+// Decryptor::invariant_noise_budget (S/decryptor.cpp:512-527): bits of Q left above the noise norm, at least 0
+static int noise_budget(const u64 *norm, size_t words, int q_bits)
+{
+    int nb = 0;
+    for (size_t i = words; i-- > 0;)
+        if (norm[i])
+        {
+            nb = (int)(64 * i + 64 - __builtin_clzll(norm[i]));
+            break;
+        }
+    return std::max(0, q_bits - nb - 1);
+}
 long Decryptor_InvariantNoiseBudget(void *p, void *enc, int *budget)
 {
     NULLRET(p);
@@ -2865,14 +2877,7 @@ long Decryptor_InvariantNoiseBudget(void *p, void *enc, int *budget)
         std::vector<u64> norm;
         int k = 0, qbits = 0;
         noise_norm((Decryptor_ *)p, *(Ciphertext_ *)enc, norm, k, qbits);
-        int nb = 0;
-        for (size_t i = norm.size(); i-- > 0;)
-            if (norm[i])
-            {
-                nb = (int)(64 * i + 64 - __builtin_clzll(norm[i]));
-                break;
-            }
-        *budget = std::max(0, qbits - nb - 1);
+        *budget = noise_budget(norm.data(), norm.size(), qbits);
     });
 }
 // Decryptor::invariant_noise (S/decryptor.cpp:487-510, added by the Sunscreen fork): the same norm as a double,
@@ -3393,7 +3398,8 @@ long Encryptor_EncryptSymmetric(void *p, void *plaintext, bool /*save_seed*/, vo
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// BatchEncoder (S/c/batchencoder.cpp -> S/batchencoder.cpp): slot permutation on the host, NTT mod t on the GPU
+// BatchEncoder (S/c/batchencoder.cpp -> S/batchencoder.cpp): slot permutation and NTT mod t on the GPU (b200_batch_encode /
+// b200_batch_decode); the per-handle calls are batches of one
 // ---------------------------------------------------------------------------------------------------------
 long BatchEncoder_Create(void *context, void **out)
 {
@@ -3405,18 +3411,6 @@ long BatchEncoder_Create(void *context, void **out)
     auto *b = new BatchEncoder_();
     b->ctx = c;
     b->hold.bind(c);
-    const size_t n = c->parms.n, row = n >> 1, m = n << 1;
-    int logn = 0;
-    while (((size_t)1 << logn) < n)
-        logn++;
-    b->index_map.resize(n);
-    u64 pos = 1;
-    for (size_t i = 0; i < row; i++)
-    {
-        b->index_map[i] = (size_t)b200::reverse_bits((pos - 1) >> 1, logn);
-        b->index_map[row | i] = (size_t)b200::reverse_bits((m - pos - 1) >> 1, logn);
-        pos = (pos * 3) & (m - 1);
-    }
     *out = b;
     return S_OK_;
 }
@@ -3433,22 +3427,55 @@ long BatchEncoder_GetSlotCount(void *p, uint64_t *count)
     *count = ((BatchEncoder_ *)p)->ctx->parms.n;
     return S_OK_;
 }
-static void batch_encode(BatchEncoder_ *b, const std::vector<u64> &vals, Plaintext_ &dst)
+// dsts[i] <- the plaintext of row i of values [count][per] (host), one transfer each way.  The reference range-checks the
+// values only in SEAL_DEBUG builds (S/batchencoder.cpp:110-193): unsigned values are reduced mod t, signed ones lifted first.
+static void encode_rows(BatchEncoder_ *b, uint64_t count, uint64_t per, const u64 *values, bool is_signed, Plaintext_ *const *dsts)
 {
     Context_ *c = b->ctx;
     const size_t n = c->parms.n;
-    if (vals.size() > n)
+    if (per > n)
         throw InvalidArg("values_matrix size is too large");
-    std::vector<u64> slots(n, 0);
-    for (size_t i = 0; i < vals.size(); i++) // the reference range-checks the values only in SEAL_DEBUG builds
-        slots[b->index_map[i]] = vals[i] % c->parms.plain; // (S/batchencoder.cpp:118-128); its transform works mod t
-
-    std::lock_guard<std::mutex> lk(c->mu);
-    DevBuf d(c, slots);
-    dev_check(b200_plain_ntt(c->dev, d.p, 1, 1, nullptr));
-    dst.coeffs = d.download();
-    dst.parms_id = kZeroId;
-    dst.scale = 1.0;
+    if (count == 0)
+        return;
+    SeamScope scope(c);
+    BatchSlab V(c, count * per), P(c, count * n);
+    if (per)
+        dev_check(b200_memcpy_h2d(c->dev, V.p, values, count * per * sizeof(u64), cur_stream()));
+    dev_check(b200_batch_encode(c->dev, V.w(), per, is_signed ? 1 : 0, P.w(), count, cur_stream()));
+    std::vector<u64> host(count * n);
+    dev_check(b200_memcpy_d2h(c->dev, host.data(), P.p, host.size() * sizeof(u64), cur_stream()));
+    scope.wait();
+    for (uint64_t i = 0; i < count; i++)
+    {
+        Plaintext_ &dst = *dsts[i];
+        dst.coeffs.assign(host.begin() + i * n, host.begin() + (i + 1) * n);
+        dst.parms_id = kZeroId;
+        dst.scale = 1.0;
+    }
+}
+// out (host [count][n]) <- the slots of plains[i], every plaintext checked first as BatchEncoder::decode checks it; signed:
+// centred (S/batchencoder.cpp:317-360)
+static void decode_rows(BatchEncoder_ *b, uint64_t count, void *const *plains, bool is_signed, void *out)
+{
+    Context_ *c = b->ctx;
+    const size_t n = c->parms.n;
+    std::vector<u64> host(count * n);
+    for (uint64_t i = 0; i < count; i++)
+    {
+        const Plaintext_ &pl = *(const Plaintext_ *)plains[i];
+        if (pl.parms_id != kZeroId)
+            throw InvalidArg("plain cannot be in NTT form");
+        std::vector<u64> v = padded_plain(c, pl);
+        std::copy(v.begin(), v.end(), host.begin() + i * n);
+    }
+    if (count == 0)
+        return;
+    SeamScope scope(c);
+    BatchSlab P(c, count * n), S(c, count * n);
+    dev_check(b200_memcpy_h2d(c->dev, P.p, host.data(), host.size() * sizeof(u64), cur_stream()));
+    dev_check(b200_batch_decode(c->dev, P.w(), is_signed ? 1 : 0, S.w(), count, cur_stream()));
+    dev_check(b200_memcpy_d2h(c->dev, out, S.p, count * n * sizeof(u64), cur_stream()));
+    scope.wait();
 }
 long BatchEncoder_Encode1(void *p, uint64_t count, uint64_t *values, void *destination)
 {
@@ -3456,7 +3483,8 @@ long BatchEncoder_Encode1(void *p, uint64_t count, uint64_t *values, void *desti
     NULLRET(destination);
     if (count)
         NULLRET(values);
-    return guard([&] { batch_encode((BatchEncoder_ *)p, std::vector<u64>(values, values + count), *(Plaintext_ *)destination); });
+    Plaintext_ *dst = (Plaintext_ *)destination;
+    return guard([&] { encode_rows((BatchEncoder_ *)p, 1, count, values, false, &dst); });
 }
 long BatchEncoder_Encode2(void *p, uint64_t count, int64_t *values, void *destination)
 {
@@ -3464,33 +3492,8 @@ long BatchEncoder_Encode2(void *p, uint64_t count, int64_t *values, void *destin
     NULLRET(destination);
     if (count)
         NULLRET(values);
-    auto *b = (BatchEncoder_ *)p;
-    return guard([&] {
-        const u64 t = b->ctx->parms.plain;
-        std::vector<u64> v(count);
-        for (uint64_t i = 0; i < count; i++)
-        {
-            const int64_t x = values[i]; // range check only in SEAL_DEBUG builds (S/batchencoder.cpp:163-175)
-            v[i] = x < 0 ? t + (u64)x : (u64)x;
-        }
-        batch_encode(b, v, *(Plaintext_ *)destination);
-    });
-}
-static std::vector<u64> batch_decode(BatchEncoder_ *b, const Plaintext_ &pl)
-{
-    Context_ *c = b->ctx;
-    const size_t n = c->parms.n;
-    if (pl.parms_id != kZeroId)
-        throw InvalidArg("plain cannot be in NTT form");
-    std::vector<u64> v = padded_plain(c, pl);
-    std::vector<u64> out(n);
-    std::lock_guard<std::mutex> lk(c->mu);
-    DevBuf d(c, v);
-    dev_check(b200_plain_ntt(c->dev, d.p, 1, 0, nullptr));
-    std::vector<u64> f = d.download();
-    for (size_t i = 0; i < n; i++)
-        out[i] = f[b->index_map[i]];
-    return out;
+    Plaintext_ *dst = (Plaintext_ *)destination;
+    return guard([&] { encode_rows((BatchEncoder_ *)p, 1, count, (const u64 *)values, true, &dst); });
 }
 long BatchEncoder_Decode1(void *p, void *plain, uint64_t *count, uint64_t *destination, void *)
 {
@@ -3500,9 +3503,8 @@ long BatchEncoder_Decode1(void *p, void *plain, uint64_t *count, uint64_t *desti
     NULLRET(destination);
     auto *b = (BatchEncoder_ *)p;
     return guard([&] {
-        std::vector<u64> out = batch_decode(b, *(Plaintext_ *)plain);
-        std::copy(out.begin(), out.end(), destination);
-        *count = out.size();
+        decode_rows(b, 1, &plain, false, destination);
+        *count = b->ctx->parms.n;
     });
 }
 long BatchEncoder_Decode2(void *p, void *plain, uint64_t *count, int64_t *destination, void *)
@@ -3513,11 +3515,78 @@ long BatchEncoder_Decode2(void *p, void *plain, uint64_t *count, int64_t *destin
     NULLRET(destination);
     auto *b = (BatchEncoder_ *)p;
     return guard([&] {
-        std::vector<u64> out = batch_decode(b, *(Plaintext_ *)plain);
-        const u64 t = b->ctx->parms.plain, half = t >> 1;
-        for (size_t i = 0; i < out.size(); i++)
-            destination[i] = out[i] > half ? (int64_t)out[i] - (int64_t)t : (int64_t)out[i];
-        *count = out.size();
+        decode_rows(b, 1, &plain, true, destination);
+        *count = b->ctx->parms.n;
+    });
+}
+long B200_BatchEncoder_EncodeBatch(void *encoder, uint64_t count, uint64_t values_per_item, const uint64_t *values, bool is_signed,
+                                   void **destinations)
+{
+    NULLRET(encoder);
+    NULLRET(destinations);
+    if (count && values_per_item)
+        NULLRET(values);
+    return guard([&] {
+        batch_handles(count, { destinations });
+        encode_rows((BatchEncoder_ *)encoder, count, values_per_item, values, is_signed, (Plaintext_ *const *)destinations);
+    });
+}
+long B200_BatchEncoder_DecodeBatch(void *encoder, uint64_t count, void **plains, bool is_signed, void *slots_out)
+{
+    NULLRET(encoder);
+    NULLRET(plains);
+    NULLRET(slots_out);
+    return guard([&] {
+        batch_handles(count, { plains });
+        decode_rows((BatchEncoder_ *)encoder, count, plains, is_signed, slots_out);
+    });
+}
+long B200_Decryptor_DecryptSlotsBatch(void *decryptor, void *encoder, uint64_t count, void **encs, bool is_signed, void *slots_out,
+                                      int *budgets)
+{
+    NULLRET(decryptor);
+    NULLRET(encoder);
+    NULLRET(encs);
+    NULLRET(slots_out);
+    auto *d = (Decryptor_ *)decryptor;
+    auto *c = d->ctx;
+    if (((BatchEncoder_ *)encoder)->ctx != c)
+        return E_INVALIDARG_;
+    return guard([&] {
+        batch_handles(count, { encs });
+        if (count == 0)
+            return;
+        const Ciphertext_ &first = *(const Ciphertext_ *)encs[0];
+        int lv = -1;
+        for (uint64_t i = 0; i < count; i++)
+        {
+            const Ciphertext_ &ct = *(const Ciphertext_ *)encs[i];
+            const int l = data_level(c, ct, "encrypted is not valid for encryption parameters");
+            if (ct.is_ntt_form)
+                throw InvalidArg("encrypted cannot be in NTT form");
+            if (i == 0)
+                lv = l;
+            else if (l != lv || ct.size != first.size)
+                throw InvalidArg("batch items must be ciphertexts of one size at one level");
+        }
+        SeamScope scope(c);
+        const size_t n = c->parms.n;
+        const int size = (int)first.size, k = c->level_k[lv];
+        const u64 *pw = d->powers(lv, size - 1);
+        b200::BigUInt Q(1);
+        for (int i = 0; i < k; i++)
+            Q.mul(c->parms.coeff[i]);
+        const size_t words = Q.w.size() + 1;
+        std::vector<u64> norm(budgets ? count * words : 0);
+        BatchSlab A(c, count * first.words()), S(c, count * n);
+        batch_gather(c, count, encs, A);
+        dev_check(b200_decrypt_slots(c->dev, lv, A.w(), size, pw, is_signed ? 1 : 0, S.w(), budgets ? norm.data() : nullptr,
+                                     (int)words, count, cur_stream()));
+        dev_check(b200_memcpy_d2h(c->dev, slots_out, S.p, count * n * sizeof(u64), cur_stream()));
+        scope.wait();
+        if (budgets)
+            for (uint64_t i = 0; i < count; i++)
+                budgets[i] = noise_budget(norm.data() + i * words, words, Q.bit_length());
     });
 }
 

@@ -580,7 +580,6 @@ struct BatchEncoder_
 {
     Context_ *ctx;
     CtxHold hold;
-    std::vector<size_t> index_map; // populate_matrix_reps_index_map (S/batchencoder.cpp:62-80)
 };
 
 struct Decryptor_

@@ -86,6 +86,9 @@ _SIGS = {
     "b200_decrypt": [vp, C.c_int, vp, C.c_int, vp, vp, u64, vp],
     "b200_ct_sk_phase": [vp, C.c_int, vp, C.c_int, vp, vp, u64, vp],
     "b200_noise_norm": [vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, u64, vp],
+    "b200_batch_encode": [vp, vp, u64, C.c_int, vp, u64, vp],
+    "b200_batch_decode": [vp, vp, C.c_int, vp, u64, vp],
+    "b200_decrypt_slots": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, u64, vp],
     "b200_is_transparent": [vp, C.c_int, vp, C.c_int, vp, u64, vp],
     "b200_any_nonzero": [vp, C.c_int, vp, C.c_int, vp, u64, vp],
     "b200_expand_signed": [vp, C.c_int, vp, C.c_int, vp, vp],
@@ -335,6 +338,24 @@ class B200Context:
         """norm_out_host: HOST uint64 array [batch][words] (little-endian multi-precision)."""
         self.L.call("b200_noise_norm", self.h, self._lv(level), vp(ptr(ct)), C.c_int(size), vp(ptr(sk_powers)),
                     vp(ptr(norm_out_host)), C.c_int(words), u64(batch), vp(stream))
+
+    def batch_encode(self, values, count, plain_out, items, signed=False, stream=None):
+        """values [items][count] (count <= n; int64 when signed) -> plain_out [items][n] coefficients mod t, the words of
+        BatchEncoder_Encode1 (Encode2 when signed).  For multiply-ready operands follow with plain_to_ntt."""
+        self.L.call("b200_batch_encode", self.h, vp(ptr(values)), u64(count), C.c_int(1 if signed else 0), vp(ptr(plain_out)),
+                    u64(items), vp(stream))
+
+    def batch_decode(self, plain, slots_out, items, signed=False, stream=None):
+        """plain [items][n] coefficient form -> slots_out [items][n]: uint64 mod t, or int64 centred when signed."""
+        self.L.call("b200_batch_decode", self.h, vp(ptr(plain)), C.c_int(1 if signed else 0), vp(ptr(slots_out)), u64(items),
+                    vp(stream))
+
+    def decrypt_slots(self, ct, size, sk_powers, slots_out, batch, signed=False, norm_out_host=None, words=0, level=None,
+                      stream=None):
+        """decrypt then batch_decode [batch][n] slots; with norm_out_host (HOST uint64 [batch][words]) also noise_norm, from
+        one secret-key phase (the call then returns after completion)."""
+        self.L.call("b200_decrypt_slots", self.h, self._lv(level), vp(ptr(ct)), C.c_int(size), vp(ptr(sk_powers)),
+                    C.c_int(1 if signed else 0), vp(ptr(slots_out)), vp(ptr(norm_out_host)), C.c_int(words), u64(batch), vp(stream))
 
     def is_transparent(self, ct, size, flags, batch, level=None, stream=None):
         self.L.call("b200_is_transparent", self.h, self._lv(level), vp(ptr(ct)), C.c_int(size), vp(ptr(flags)), u64(batch),
