@@ -123,6 +123,35 @@ int b200_batch_decode(b200_ctx *ctx, const uint64_t *plain, int is_signed, uint6
 int b200_decrypt_slots(b200_ctx *ctx, int level, const uint64_t *ct, int size, const uint64_t *sk_powers_ntt, int is_signed,
                        uint64_t *slots_out, uint64_t *norm_out, int words, uint64_t batch, void *stream);
 
+/* ---- encryption (S/encryptor.cpp), batched, in two steps.  The host step samples the random stream with the reference's
+   generators (sampling.h): item i from Blake2xbPrng(seeds[i]), seeds HOST [batch][8], the items in parallel on the context's
+   host threads (one item on the calling thread); it touches no device state.  Ternary and clipped-normal samples are int8.
+   The device step is one launch sequence per call whatever the batch; it is asynchronous, and the host samples must stay
+   unchanged until the stream has passed it (they are not wiped by the library: the caller owns them).  Device scratch that
+   held u, e or products with the secret key is wiped in stream order.  Device memory: about 3 n + 24 k_e n bytes of scratch
+   per pk item, 8 k n + n per sk item. ---- */
+/* u, e0, e1 of each item in the order of Encryptor_EncryptReturnComponentsSetSeed: samples_out HOST [batch][3][n] */
+int b200_sample_pk(b200_ctx *ctx, const uint64_t *seeds, int8_t *samples_out, uint64_t batch);
+/* the public seed from the bootstrap PRNG, the uniform c1 (NTT form, first data level) from it, then e, as
+   Encryptor_EncryptSymmetricReturnComponentsSetSeed draws them: c1_out HOST [batch][k1][n], noise_out HOST [batch][n] */
+int b200_sample_sk(b200_ctx *ctx, const uint64_t *seeds, uint64_t *c1_out, int8_t *noise_out, uint64_t batch);
+/* pk encryption of `batch` plaintexts from b200_sample_pk's samples.  pk: device [2][K][n] NTT form at the key level; plain:
+   device [batch][n] coefficients mod t; out: device [batch][2][k1][n] at the first data level (encrypted at the key level and
+   switched down, or with disable_special_modulus encrypted there directly) */
+int b200_encrypt_pk_samples(b200_ctx *ctx, const uint64_t *pk, const int8_t *samples, const uint64_t *plain,
+                            int disable_special_modulus, uint64_t *out, uint64_t batch, void *stream);
+/* sk encryption at the first data level from b200_sample_sk's c1 and e: c0 = -(s c1 + e) + Delta m.  sk: device [K][n] NTT
+   form.  On failure `out` is wiped (it holds s (*) c1 on the way). */
+int b200_encrypt_sk_samples(b200_ctx *ctx, const uint64_t *sk, const uint64_t *c1, const int8_t *noise, const uint64_t *plain,
+                            uint64_t *out, uint64_t batch, void *stream);
+/* both steps in one call, returning after completion: item i gives the words of Encryptor_EncryptReturnComponentsSetSeed
+   (Encryptor_EncryptSymmetricReturnComponentsSetSeed) with seeds[i]; samples_out (NULL or HOST [batch][3][n]) / noise_out
+   (NULL or HOST [batch][n]) receive the samples */
+int b200_encrypt_pk(b200_ctx *ctx, const uint64_t *pk, const uint64_t *seeds, const uint64_t *plain, int disable_special_modulus,
+                    uint64_t *out, int8_t *samples_out, uint64_t batch, void *stream);
+int b200_encrypt_sk(b200_ctx *ctx, const uint64_t *sk, const uint64_t *seeds, const uint64_t *plain, uint64_t *out,
+                    int8_t *noise_out, uint64_t batch, void *stream);
+
 /* ---- ciphertext arithmetic, batched over `batch` independent items (device pointers) ---- */
 int b200_add(b200_ctx *ctx, int level, const uint64_t *a, const uint64_t *b, uint64_t *out, int size, uint64_t batch,
              void *stream);

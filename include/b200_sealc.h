@@ -339,6 +339,23 @@ SEAL_C_FUNC B200_BatchEncoder_EncodeBatch(void *encoder, uint64_t count, uint64_
 SEAL_C_FUNC B200_BatchEncoder_DecodeBatch(void *encoder, uint64_t count, void **plains, bool is_signed, void *slots_out);
 SEAL_C_FUNC B200_Decryptor_DecryptSlotsBatch(void *decryptor, void *encoder, uint64_t count, void **encrypteds, bool is_signed,
                                              void *slots_out, int *budgets);
+/* encryption of many plaintexts at once: every item is sampled on the host from its own seed, in parallel over items, and the
+   samples cross in one int8 transfer; the arithmetic is one launch sequence per call.
+   EncryptBatch: destinations[i] receives Encryptor_Encrypt(plains[i]) (symmetric: Encryptor_EncryptSymmetric).  seeds: host
+   [count][8], item i then gives the words of B200_Encryptor_EncryptSetSeed(plains[i], seeds + 8 i) (symmetric: of
+   Encryptor_EncryptSymmetricReturnComponentsSetSeed), or NULL for a fresh random seed per item.  Same checks and HRESULTs
+   as those calls, all made before any work (a missing key first, then the plaintexts).
+   EncryptSlotsBatch: the same for the plaintexts B200_BatchEncoder_EncodeBatch gives for `values` (host
+   [count][values_per_item], int64_t when is_signed), encoded on the device with no plaintext handles in between: the mirror
+   of DecryptSlotsBatch.  Same checks and HRESULTs as EncodeBatch and EncryptBatch, all made before any work, except: an
+   encoder of another context, and parameters that do not batch, are E_INVALIDARG.
+   Destinations must be distinct (E_INVALIDARG).  Destinations are untouched when a call is refused.  The sampling runs
+   before the call takes the context, so other threads' operations proceed meanwhile. */
+SEAL_C_FUNC B200_Encryptor_EncryptBatch(void *encryptor, uint64_t count, void **plains, const uint64_t *seeds, bool symmetric,
+                                        void **destinations);
+SEAL_C_FUNC B200_Encryptor_EncryptSlotsBatch(void *encryptor, void *encoder, uint64_t count, uint64_t values_per_item,
+                                             const uint64_t *values, bool is_signed, const uint64_t *seeds, bool symmetric,
+                                             void **destinations);
 
 /* ---- debug aids (tests only; not part of the seal_fhe surface) ---- */
 /* `count` (1 ... 64) per-handle calls of one kind run as if they had arrived together at the combiner: kind 0

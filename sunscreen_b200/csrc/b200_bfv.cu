@@ -7,6 +7,7 @@
 #include "../../include/b200_bfv.h"
 #include "bfv_body.cuh"
 #include "host_ctx.h"
+#include "sampling.h"
 #include "ntt_body.cuh"
 #include "ntt_fp_body.cuh"
 #include <atomic>
@@ -1243,6 +1244,97 @@ __global__ void slot_gather_kernel(const u32 *map, u64 t, const u64 *plain, int 
     slots[idx] = is_signed && v > (t >> 1) ? v - t : v;
 }
 
+// ---- encryption around the transforms (b200_encrypt_pk / b200_encrypt_sk); the small host samples arrive as int8 ----
+B200_HD u64 small_residue(int8_t v, u64 p) { return v < 0 ? p + (u64)(long long)v : (u64)v; }
+
+// out[item][r][c] = residue r of vals[item * val_item + c]
+__global__ void expand_int8_kernel(const PrimeDev *primes, int k, const int8_t *vals, long long val_item, u64 *out, int logn,
+                                   long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long c = idx & ((1LL << logn) - 1), t = idx >> logn;
+    const int r = (int)(t % k);
+    out[idx] = small_residue(vals[(t / k) * val_item + c], __ldg(&primes[r].p));
+}
+
+// out[item][j][r][c] = key[j][r][c] * x[item][r][c] mod q_r for j < polys (key polys `key_poly` words apart, so a [2][K][n]
+// public key serves any prefix of its residues); x_copy != NULL also receives x in the rows after the product (sk: c1)
+__global__ void enc_dyadic_kernel(const PrimeDev *primes, int k, int polys, const u64 *key, long long key_poly, const u64 *x,
+                                  long long x_item, u64 *out, long long out_item, u64 *x_copy, int logn, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long n = 1LL << logn, c = idx & (n - 1), t = idx >> logn;
+    const int r = (int)(t % k);
+    const long long u = t / k, item = u / polys;
+    const int j = (int)(u % polys);
+    const PrimeDev P = ld_prime(&primes[r]);
+    const u64 xv = x[item * x_item + r * n + c];
+    u64 lo, hi;
+    mul128(__ldg(&key[j * key_poly + r * n + c]), xv, lo, hi);
+    out[item * out_item + ((long long)j * k + r) * n + c] = barrett128(lo, hi, P.p, P.r0, P.r1);
+    if (x_copy)
+        x_copy[item * out_item + r * n + c] = xv;
+}
+
+// Encryption tail at the output level, no modulus switch: poly j < polys of item i becomes src + e_j, negated when `negate`
+// (sk: c0 = -(s c1 + e)), and poly 0 then gains Delta m by addsub_plain_kernel's rule.  src and out: [batch][2][k][n] (they may
+// alias); e_j: e[item * e_item + j * n].
+__global__ void enc_tail_kernel(const LevelDev L, const u64 *src, const int8_t *e, long long e_item, const u64 *plain, u64 *out,
+                                int polys, int negate, int logn, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long n = 1LL << logn, c = idx & (n - 1), t = idx >> logn;
+    const int r = (int)(t % L.k);
+    const long long u = t / L.k, item = u / polys;
+    const int j = (int)(u % polys);
+    const PrimeDev Q = ld_prime(&L.q[r]);
+    const long long at = (item * 2 + j) * L.k * n + r * n + c;
+    u64 v = add_mod(src[at], small_residue(e[item * e_item + j * n + c], Q.p), Q.p);
+    if (negate)
+        v = neg_mod(v, Q.p);
+    if (j == 0)
+        v = add_mod(v, plain_scaled(L, Q, r, plain[item * n + c]), Q.p);
+    out[at] = v;
+}
+
+// pk encryption tail with the special prime dropped: x = INTT(pk_j u) + e_j at the key level (K residues), divided and rounded
+// by the last prime as modswitch_kernel does, then Delta m added to poly 0 at the first data level L1.  One thread per
+// (item, poly, coefficient); samples: [batch][3][n] (u, e0, e1), out: [batch][2][K-1][n].
+template <int K>
+__global__ void enc_pk_drop_tail_kernel(const PrimeDev *primes, const u64 *inv_qlast, const LevelDev L1, const u64 *x,
+                                        const int8_t *samples, const u64 *plain, u64 *out, int logn, long long total)
+{
+    const long long idx = GLOBAL_IDX();
+    if (idx >= total)
+        return;
+    const long long n = 1LL << logn, c = idx & (n - 1), u = idx >> logn, item = u >> 1;
+    const int j = (int)(u & 1);
+    const int8_t ev = samples[(item * 3 + 1 + j) * n + c];
+    const u64 m = j == 0 ? plain[item * n + c] : 0;
+    const u64 *src = x + u * K * n + c;
+    u64 *dst = out + u * (K - 1) * n + c;
+    modswitch_body<K>(
+        primes, inv_qlast,
+        [&](int i) {
+            const u64 p = __ldg(&primes[i].p);
+            return add_mod(src[i * n], small_residue(ev, p), p);
+        },
+        [&](int i, u64 v) {
+            if (j == 0)
+            {
+                const PrimeDev Q = ld_prime(&L1.q[i]);
+                v = add_mod(v, plain_scaled(L1, Q, i, m), Q.p);
+            }
+            dst[i * n] = v;
+        });
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------------------
@@ -1274,11 +1366,12 @@ struct FpMasks
     int running = 0; // the schedule whose masks the transforms use
 };
 
-// minimal fork-join pool (the packing loops are pure streaming work; 8-16 threads saturate what PCIe can take)
+// minimal fork-join pool (the packing loops are pure streaming work; 8-16 threads saturate what PCIe can take; encryption
+// samples its items on it, each from its own PRNG)
 struct HostPool
 {
     std::vector<std::thread> th;
-    std::mutex mu;
+    std::mutex mu, run_mu;
     std::condition_variable cv_work, cv_done;
     std::function<void(int, int)> task;
     long long generation = 0;
@@ -1324,6 +1417,7 @@ struct HostPool
     }
     void run(const std::function<void(int, int)> &fn)
     {
+        std::lock_guard<std::mutex> one(run_mu); // one task at a time: callers on other threads wait their turn
         if (nth == 1)
         {
             fn(0, 1);
@@ -1466,7 +1560,7 @@ struct b200_ctx
     cudaEvent_t ev_fork = nullptr, ev_join[NSIDE] = { nullptr, nullptr, nullptr, nullptr };
     int mr_split = 1;
     StagingRing ring;
-    std::unique_ptr<HostPool> pool; // packing threads of the packed staging (created on first use)
+    std::unique_ptr<HostPool> pool; // threads of the packed staging and of encryption's sampling (created on first use)
     int ntt_threads = 256;
     size_t ntt_smem = 0;
     int ntt_split = 0; // n > 16384: two-level transform, ntt_outer_kernel + 2^split sub-transforms of n >> split points
@@ -3126,6 +3220,268 @@ int b200_batch_decode(b200_ctx *ctx, const uint64_t *plain, int is_signed, uint6
     return slots_from_plain(ctx, (const u64 *)plain, work, is_signed, (u64 *)slots_out, (long long)items, s);
 }
 
+// ---- encryption (S/encryptor.cpp, S/util/rlwe.cpp) in two steps: the host sampling (b200_sample_pk / b200_sample_sk), which
+// touches no device state, then the device work on the samples (b200_encrypt_pk_samples / b200_encrypt_sk_samples), one launch
+// sequence per call ----
+static HostPool *host_pool(b200_ctx *ctx);
+
+// one zero "modulus": the samplers of sampling.h then return the small signed value itself, as a two's-complement word
+static const std::vector<uint64_t> one_zero(1, 0);
+
+// the samplers' two's-complement words as int8 (ternary values are in {-1, 0, 1}, clipped-normal ones truncations of
+// |x| <= 19.2); false when one does not fit
+static bool narrow_small(const uint64_t *v, long long n, int8_t *dst)
+{
+    bool ok = true;
+    for (long long c = 0; c < n; c++)
+    {
+        const long long x = (long long)v[c];
+        ok &= x >= -128 && x <= 127;
+        dst[c] = (int8_t)x;
+    }
+    return ok;
+}
+
+// sample(i, tmp) draws item i (tmp: n words of scratch, wiped afterwards).  One item is drawn on the calling thread, so that
+// threads encrypting one item each sample at the same time; a batch is spread over the host pool's threads.
+static int sample_items(b200_ctx *ctx, uint64_t batch, const std::function<bool(uint64_t, uint64_t *)> &sample)
+{
+    std::atomic<bool> ok{ true };
+    auto work = [&](int id, int nth) {
+        std::vector<uint64_t> tmp(ctx->n);
+        for (uint64_t i = (uint64_t)id; i < batch; i += (uint64_t)nth)
+            if (!sample(i, tmp.data()))
+                ok = false;
+        explicit_bzero(tmp.data(), tmp.size() * sizeof(uint64_t));
+    };
+    if (batch == 1)
+        work(0, 1);
+    else
+        host_pool(ctx)->run(work);
+    return ok ? 0 : fail(B200_E_LOGIC, "internal: a small sample does not fit int8");
+}
+
+static b200::PrngSeed seed_of(const uint64_t *seeds, uint64_t i)
+{
+    b200::PrngSeed sd;
+    std::copy_n(seeds + 8 * i, 8, sd.begin());
+    return sd;
+}
+
+int b200_sample_pk(b200_ctx *ctx, const uint64_t *seeds, int8_t *samples_out, uint64_t batch)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if (!seeds || !samples_out)
+        return fail(B200_E_NULL, "null pointer");
+    const long long n = (long long)ctx->n;
+    // per item u, e0, e1 in the order of encrypt_zero_asymmetric (S/util/rlwe.cpp:193-310)
+    return sample_items(ctx, batch, [&](uint64_t i, uint64_t *tmp) {
+        b200::Blake2xbPrng prng(seed_of(seeds, i));
+        int8_t *d = samples_out + (size_t)i * 3 * n;
+        b200::sample_poly_ternary(prng, (size_t)n, one_zero, tmp);
+        bool ok = narrow_small(tmp, n, d);
+        b200::sample_poly_normal(prng, (size_t)n, one_zero, tmp);
+        ok &= narrow_small(tmp, n, d + n);
+        b200::sample_poly_normal(prng, (size_t)n, one_zero, tmp);
+        return narrow_small(tmp, n, d + 2 * n) && ok;
+    });
+}
+
+int b200_sample_sk(b200_ctx *ctx, const uint64_t *seeds, uint64_t *c1_out, int8_t *noise_out, uint64_t batch)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if (!seeds || !c1_out || !noise_out)
+        return fail(B200_E_NULL, "null pointer");
+    const int lv = ctx->host->first_level();
+    const long long n = (long long)ctx->n, k = ctx->levels[lv].k;
+    std::vector<uint64_t> mods;
+    for (int idx : ctx->host->levels[lv].q_idx)
+        mods.push_back(ctx->host->primes[idx].mod.p);
+    // per item: the public seed, the uniform c1 from it, then e (encrypt_zero_symmetric, S/util/rlwe.cpp:312-459)
+    return sample_items(ctx, batch, [&](uint64_t i, uint64_t *tmp) {
+        b200::Blake2xbPrng bootstrap(seed_of(seeds, i));
+        b200::PrngSeed pub;
+        bootstrap.generate(sizeof(pub), pub.data());
+        b200::Blake2xbPrng ct_prng(pub);
+        b200::sample_poly_uniform(ct_prng, (size_t)n, mods, c1_out + (size_t)i * k * n);
+        b200::sample_poly_normal(bootstrap, (size_t)n, one_zero, tmp);
+        return narrow_small(tmp, n, noise_out + (size_t)i * n);
+    });
+}
+
+// zeroes the device buffers in stream order before Scratch releases them
+static void wipe_async(const std::vector<std::pair<void *, size_t>> &bufs, cudaStream_t s)
+{
+    for (auto &w : bufs)
+        if (w.first)
+            cudaMemsetAsync(w.first, 0, w.second, s);
+}
+
+int b200_encrypt_pk_samples(b200_ctx *ctx, const uint64_t *pk, const int8_t *samples, const uint64_t *plain,
+                            int disable_special_modulus, uint64_t *out, uint64_t batch, void *stream)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if (!pk || !samples || !plain || !out)
+        return fail(B200_E_NULL, "null pointer");
+    if (batch == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    const int lv = ctx->host->first_level(), K = ctx->host->K;
+    const bool drop = lv == 1 && !disable_special_modulus; // encrypt at the key level, then switch down
+    const int enc = drop ? 0 : lv, ke = ctx->levels[enc].k;
+    const long long n = (long long)ctx->n, B = (long long)batch;
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    std::vector<std::pair<void *, size_t>> wipe; // everything that holds u, e or a product with them
+    u64 *d8 = nullptr, *du = nullptr, *dx = nullptr;
+    int rc = 0;
+    auto run = [&]() -> int {
+        int rc2;
+        if ((rc2 = scr.get((size_t)(B * 3 * n + 7) / 8, &d8)))
+            return rc2;
+        wipe.emplace_back(d8, (size_t)B * 3 * n);
+        if ((rc2 = scr.get((size_t)B * ke * n, &du)))
+            return rc2;
+        wipe.emplace_back(du, (size_t)B * ke * n * 8);
+        if ((rc2 = scr.get((size_t)B * 2 * ke * n, &dx)))
+            return rc2;
+        wipe.emplace_back(dx, (size_t)B * 2 * ke * n * 8);
+        CU_TRY(cudaMemcpyAsync(d8, samples, (size_t)B * 3 * n, cudaMemcpyHostToDevice, s));
+        const int8_t *smp = (const int8_t *)d8;
+        long long total = B * ke * n;
+        B200_LAUNCH(expand_int8_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, ke, smp, 3 * n, du, ctx->logn, total);
+        ctx->launches++;
+        if ((rc2 = ntt_slab(ctx, enc, du, batch, s, true)))
+            return rc2;
+        total = B * 2 * ke * n;
+        B200_LAUNCH(enc_dyadic_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, ke, 2, (const u64 *)pk, (long long)K * n,
+                    (const u64 *)du, (long long)ke * n, dx, 2LL * ke * n, (u64 *)nullptr, ctx->logn, total);
+        ctx->launches++;
+        if ((rc2 = ntt_slab(ctx, enc, dx, 2 * batch, s, false))) // pk_j (*) NTT(u) back to coefficients: 2 batch polys
+            return rc2;
+        if (drop)
+        {
+            total = B * 2 * n;
+            // 17 residues: the key level of a chain with 16 data residues (modswitch_coeff is integer-only, as in
+            // b200_mod_switch_to_next)
+            if (K == 17)
+                B200_LAUNCH(enc_pk_drop_tail_kernel<17>, blocks_for(total, EB), EB, 0, s, ctx->d_primes, ctx->levels[0].inv_qlast,
+                            ctx->levels[lv], (const u64 *)dx, smp, (const u64 *)plain, (u64 *)out, ctx->logn, total);
+            else
+                DISPATCH_K(K, B200_LAUNCH(enc_pk_drop_tail_kernel<KK>, blocks_for(total, EB), EB, 0, s, ctx->d_primes,
+                                          ctx->levels[0].inv_qlast, ctx->levels[lv], (const u64 *)dx, smp, (const u64 *)plain,
+                                          (u64 *)out, ctx->logn, total));
+        }
+        else
+            B200_LAUNCH(enc_tail_kernel, blocks_for(total, EB), EB, 0, s, ctx->levels[lv], (const u64 *)dx, smp + n, 3 * n,
+                        (const u64 *)plain, (u64 *)out, 2, 0, ctx->logn, total);
+        ctx->launches++;
+        CU_TRY(cudaGetLastError());
+        return 0;
+    };
+    rc = run();
+    wipe_async(wipe, s);
+    return rc;
+}
+
+int b200_encrypt_sk_samples(b200_ctx *ctx, const uint64_t *sk, const uint64_t *c1, const int8_t *noise, const uint64_t *plain,
+                            uint64_t *out, uint64_t batch, void *stream)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if (!sk || !c1 || !noise || !plain || !out)
+        return fail(B200_E_NULL, "null pointer");
+    if (batch == 0)
+        return 0;
+    CU_TRY(cudaSetDevice(ctx->device));
+    const int lv = ctx->host->first_level(), k = ctx->levels[lv].k;
+    const long long n = (long long)ctx->n, B = (long long)batch;
+    cudaStream_t s = (cudaStream_t)stream;
+    Scratch scr(ctx, s);
+    std::vector<std::pair<void *, size_t>> wipe;
+    u64 *dc1 = nullptr, *de = nullptr;
+    u64 *o = (u64 *)out;
+    bool products = false; // out holds s (*) c1 until the tail has run
+    auto run = [&]() -> int {
+        int rc2;
+        if ((rc2 = scr.get((size_t)B * k * n, &dc1)) || (rc2 = scr.get((size_t)(B * n + 7) / 8, &de)))
+            return rc2;
+        wipe.emplace_back(de, (size_t)B * n);
+        CU_TRY(cudaMemcpyAsync(dc1, c1, (size_t)B * k * n * 8, cudaMemcpyHostToDevice, s));
+        CU_TRY(cudaMemcpyAsync(de, noise, (size_t)B * n, cudaMemcpyHostToDevice, s));
+        // c0 rows <- s (*) c1 and c1 rows <- c1, both NTT form; then both back to coefficients
+        long long total = B * k * n;
+        products = true;
+        B200_LAUNCH(enc_dyadic_kernel, blocks_for(total, EB), EB, 0, s, ctx->d_primes, k, 1, (const u64 *)sk, 0LL, (const u64 *)dc1,
+                    (long long)k * n, o, 2LL * k * n, o + (long long)k * n, ctx->logn, total);
+        ctx->launches++;
+        if ((rc2 = ntt_slab(ctx, lv, o, 2 * batch, s, false)))
+            return rc2;
+        B200_LAUNCH(enc_tail_kernel, blocks_for(total, EB), EB, 0, s, ctx->levels[lv], (const u64 *)o, (const int8_t *)de, n,
+                    (const u64 *)plain, o, 1, 1, ctx->logn, total);
+        ctx->launches++;
+        CU_TRY(cudaGetLastError());
+        return 0;
+    };
+    const int rc = run();
+    if (rc && products)
+        wipe.emplace_back(o, (size_t)B * 2 * k * n * 8);
+    wipe_async(wipe, s);
+    return rc;
+}
+
+// sampling and device work in one call; returns after completion, with the host copy of the samples wiped
+int b200_encrypt_pk(b200_ctx *ctx, const uint64_t *pk, const uint64_t *seeds, const uint64_t *plain, int disable_special_modulus,
+                    uint64_t *out, int8_t *samples_out, uint64_t batch, void *stream)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if (!pk || !seeds || !plain || !out)
+        return fail(B200_E_NULL, "null pointer");
+    if (batch == 0)
+        return 0;
+    std::vector<int8_t> smp((size_t)batch * 3 * ctx->n);
+    int rc = b200_sample_pk(ctx, seeds, smp.data(), batch);
+    if (!rc && samples_out)
+        std::memcpy(samples_out, smp.data(), smp.size());
+    if (!rc)
+        rc = b200_encrypt_pk_samples(ctx, pk, smp.data(), plain, disable_special_modulus, out, batch, stream);
+    const cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
+    explicit_bzero(smp.data(), smp.size());
+    if (rc)
+        return rc;
+    CU_TRY(e);
+    return 0;
+}
+
+int b200_encrypt_sk(b200_ctx *ctx, const uint64_t *sk, const uint64_t *seeds, const uint64_t *plain, uint64_t *out,
+                    int8_t *noise_out, uint64_t batch, void *stream)
+{
+    if (!ctx)
+        return fail(B200_E_NULL, "null context");
+    if (!sk || !seeds || !plain || !out)
+        return fail(B200_E_NULL, "null pointer");
+    if (batch == 0)
+        return 0;
+    const size_t n = ctx->n, k = (size_t)ctx->levels[ctx->host->first_level()].k;
+    std::vector<uint64_t> c1((size_t)batch * k * n);
+    std::vector<int8_t> noise((size_t)batch * n);
+    int rc = b200_sample_sk(ctx, seeds, c1.data(), noise.data(), batch);
+    if (!rc && noise_out)
+        std::memcpy(noise_out, noise.data(), noise.size());
+    if (!rc)
+        rc = b200_encrypt_sk_samples(ctx, sk, c1.data(), noise.data(), plain, out, batch, stream);
+    const cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
+    explicit_bzero(noise.data(), noise.size());
+    if (rc)
+        return rc;
+    CU_TRY(e);
+    return 0;
+}
+
 // ---- add / sub / negate ----
 static int addsub(b200_ctx *ctx, int level, const u64 *a, const u64 *b, u64 *out, int size, uint64_t batch, void *stream,
                   int mode)
@@ -4365,6 +4721,7 @@ __global__ void pack48_kernel(const u64 *in, u64 *packed, long long groups)
 
 static HostPool *host_pool(b200_ctx *ctx)
 {
+    std::lock_guard<std::mutex> lk(ctx->mu); // the packed pipeline and encryption may ask for it at once
     if (!ctx->pool)
     {
         int n = 0;

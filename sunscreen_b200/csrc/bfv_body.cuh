@@ -293,13 +293,13 @@ B200_HD void ksmac_coeff(const PrimeDev &P, const u64 *__restrict__ ops, long lo
 // ---------------------------------------------------------------------------------------------------------
 // divide-and-round by the last prime (BFV mod switch): rows [K] -> [K-1]
 // ---------------------------------------------------------------------------------------------------------
-template <int K>
-B200_HD void modswitch_coeff(const PrimeDev *__restrict__ q, const u64 *__restrict__ inv_qlast, const u64 *__restrict__ src,
-                             long long n, u64 *__restrict__ dst, long long c)
+// ld(i): canonical residue i of the coefficient (the last one is read first); st(i, v): result residue i < K - 1
+template <int K, class Ld, class St>
+B200_HD void modswitch_body(const PrimeDev *__restrict__ q, const u64 *__restrict__ inv_qlast, Ld ld, St st)
 {
     const PrimeDev LP = ld_prime(&q[K - 1]);
     const u64 half = LP.p >> 1;
-    u64 s = src[(K - 1) * n + c] + half;
+    u64 s = ld(K - 1) + half;
     s = s >= LP.p ? s - LP.p : s;
 #pragma unroll
     for (int i = 0; i < K - 1; i++)
@@ -307,9 +307,16 @@ B200_HD void modswitch_coeff(const PrimeDev *__restrict__ q, const u64 *__restri
         const PrimeDev Q = ld_prime(&q[i]);
         const u64 r = barrett64(s, Q.p, Q.r1);
         const u64 h = barrett64(half, Q.p, Q.r1);
-        u64 v = src[i * n + c] + (Q.p - r) + h;
-        dst[i * n + c] = shoup_mul(v, B200_LDG(&inv_qlast[2 * i]), B200_LDG(&inv_qlast[2 * i + 1]), Q.p);
+        u64 v = ld(i) + (Q.p - r) + h;
+        st(i, shoup_mul(v, B200_LDG(&inv_qlast[2 * i]), B200_LDG(&inv_qlast[2 * i + 1]), Q.p));
     }
+}
+
+template <int K>
+B200_HD void modswitch_coeff(const PrimeDev *__restrict__ q, const u64 *__restrict__ inv_qlast, const u64 *__restrict__ src,
+                             long long n, u64 *__restrict__ dst, long long c)
+{
+    modswitch_body<K>(q, inv_qlast, [&](int i) { return src[i * n + c]; }, [&](int i, u64 v) { dst[i * n + c] = v; });
 }
 
 // ---------------------------------------------------------------------------------------------------------

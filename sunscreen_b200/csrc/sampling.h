@@ -7,7 +7,7 @@
 //   sample_poly_normal     S/util/rlwe.cpp:43-67    (ClippedNormalDistribution: std::normal_distribution, sigma 3.2, clip 19.2)
 //   sample_poly_uniform    S/util/rlwe.cpp:107-135  (rejection below the largest multiple of the modulus)
 // The std:: distributions are used as such (same libstdc++ as the reference build), only the engine is ours.
-// The arithmetic around the samples (NTT, dyadic products, additions) runs on the GPU (sealc_api.cpp).
+// The arithmetic around the samples (NTT, dyadic products, additions) runs on the GPU (b200_bfv.cu, sealc_api.cpp).
 #pragma once
 #include <array>
 #include <cstddef>

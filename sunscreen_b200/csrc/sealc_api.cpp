@@ -3163,6 +3163,115 @@ long Encryptor_Destroy(void *p)
     return S_OK_;
 }
 
+// Encryption (S/encryptor.cpp:160-321) in two steps: the host sampling (b200_sample_pk / b200_sample_sk), done before the
+// operation scope so that it holds no lock of the context — threads that encrypt at the same time sample in parallel and
+// serialise only for the device part — then one launch sequence for the batch (b200_encrypt_pk_samples / _sk_samples).  Every
+// entry point, per-handle ones included, is a batch.  The key is checked before the plaintexts, as the reference checks them.
+static void encrypt_key_check(Encryptor_ *e, bool symmetric)
+{
+    if (symmetric ? !e->has_sk : !e->has_pk)
+        throw LogicErr(symmetric ? "secret key is not set" : "public key is not set");
+}
+// plains[i] padded to n coefficients, host [count][n], each checked as Encryptor::encrypt checks it (is_valid_for)
+static std::vector<u64> encrypt_plains(Context_ *c, uint64_t count, void *const *plains)
+{
+    const size_t n = c->parms.n;
+    std::vector<u64> host(count * n);
+    for (uint64_t i = 0; i < count; i++)
+    {
+        std::vector<u64> v = padded_plain(c, *(const Plaintext_ *)plains[i]);
+        std::copy(v.begin(), v.end(), host.begin() + i * n);
+    }
+    return host;
+}
+// a batch seam writes each destination once: a handle listed twice is refused (the scatter writes the items concurrently)
+static void distinct_destinations(uint64_t count, void *const *dsts)
+{
+    std::vector<void *> v(dsts, dsts + count);
+    std::sort(v.begin(), v.end());
+    if (std::adjacent_find(v.begin(), v.end()) != v.end())
+        throw InvalidArg("destinations must be distinct");
+}
+// The host samples of one call: pk u, e0, e1 ([count][3][n]) or sk e ([count][n]) and c1 ([count][k][n], public).  The small
+// samples, and the seeds drawn for an unseeded call (which determine them), are wiped when the call is done.
+struct EncSamples
+{
+    std::vector<int8_t> small;
+    std::vector<u64> c1, seeds;
+    ~EncSamples()
+    {
+        explicit_bzero(small.data(), small.size());
+        wipe(seeds);
+    }
+};
+// seeds: host [count][8], or NULL for a fresh random seed per item
+static void encrypt_sample(Context_ *c, uint64_t count, const uint64_t *seeds, bool symmetric, EncSamples &S)
+{
+    const size_t n = c->parms.n, k = (size_t)c->level_k[c->first_level];
+    if (!seeds)
+    {
+        S.seeds.resize(count * 8);
+        for (uint64_t i = 0; i < count; i++)
+        {
+            b200::PrngSeed sd = b200::random_seed();
+            std::copy(sd.begin(), sd.end(), S.seeds.begin() + i * 8);
+            explicit_bzero(sd.data(), sizeof(sd));
+        }
+        seeds = S.seeds.data();
+    }
+    if (symmetric)
+    {
+        S.c1.resize(count * k * n);
+        S.small.resize(count * n);
+        dev_check(b200_sample_sk(c->dev, seeds, S.c1.data(), S.small.data(), count));
+    }
+    else
+    {
+        S.small.resize(count * 3 * n);
+        dev_check(b200_sample_pk(c->dev, seeds, S.small.data(), count));
+    }
+}
+// dsts[i] <- the encryption of plaintext row i of the device slab P [count][n] (checked) with the samples S, at the first data
+// level.  Runs inside the caller's SeamScope; the caller waits before S goes away.
+static void encrypt_device(Encryptor_ *e, uint64_t count, const BatchSlab &P, const EncSamples &S, bool symmetric, bool dsm,
+                           void *const *dsts)
+{
+    Context_ *c = e->ctx;
+    const int lv = c->first_level;
+    const u64 k = (u64)c->level_k[lv], w = 2 * k * c->parms.n;
+    // one item is encrypted straight into its destination; a batch into a slab, then scattered
+    std::unique_ptr<BatchSlab> O(count > 1 ? new BatchSlab(c, count * w) : nullptr);
+    u64 *out = O ? O->w() : ((Ciphertext_ *)dsts[0])->prepare_output(c, c->ids[lv], 2, k);
+    if (symmetric)
+        dev_check(b200_encrypt_sk_samples(c->dev, e->dev_sk(), S.c1.data(), S.small.data(), P.w(), out, count, cur_stream()));
+    else
+        dev_check(b200_encrypt_pk_samples(c->dev, e->dev_pk(), S.small.data(), P.w(), dsm ? 1 : 0, out, count, cur_stream()));
+    if (!O)
+        return;
+    std::vector<u64 *> ptrs(count);
+    for (uint64_t i = 0; i < count; i++)
+        ptrs[i] = ((Ciphertext_ *)dsts[i])->prepare_output(c, c->ids[lv], 2, k);
+    const uint64_t chunk = 65535; // items per b200_gather_scatter
+    for (uint64_t i0 = 0; i0 < count; i0 += chunk)
+        dev_check(b200_gather_scatter(c->dev, ptrs.data() + i0, std::min(chunk, count - i0), O->w() + i0 * w, w, 0, cur_stream()));
+}
+// plaintext handles -> ciphertexts, every item checked before any work; S receives the samples
+static void encrypt_batch(Encryptor_ *e, uint64_t count, void *const *plains, const uint64_t *seeds, bool symmetric, bool dsm,
+                          void *const *dsts, EncSamples &S)
+{
+    Context_ *c = e->ctx;
+    encrypt_key_check(e, symmetric);
+    const std::vector<u64> host = encrypt_plains(c, count, plains);
+    if (count == 0)
+        return;
+    encrypt_sample(c, count, seeds, symmetric, S);
+    SeamScope scope(c);
+    BatchSlab P(c, host.size());
+    dev_check(b200_memcpy_h2d(c->dev, P.p, host.data(), host.size() * sizeof(u64), cur_stream()));
+    encrypt_device(e, count, P, S, symmetric, dsm, dsts);
+    scope.wait(); // the device has read the samples
+}
+
 // Components of an encryption as the reference exports them (S/util/rlwe.cpp:243-288,403-407; S/util/scalingvariant.cpp:96-119)
 struct EncComponents
 {
@@ -3183,131 +3292,40 @@ static void export_remainder(Context_ *c, const Plaintext_ &plain, Plaintext_ &d
     dst = std::move(r);
 }
 
-// pk encryption of `plain` with the given PRNG: encrypt_zero_asymmetric at the key level, divide-and-round by the
-// special prime, then add round(q m / t) (S/util/rlwe.cpp:193-310, S/encryptor.cpp:160-208,300-312).  With
-// `disable_special_modulus` the zero encryption is made directly at the first data level from the first k residues
-// of the public key and no modulus switch follows (S/encryptor.cpp:160-163,210-224).
-// `lk` (the context mutex, not yet held) is taken only after the host-side sampling, which touches nothing shared: threads
-// that encrypt concurrently sample in parallel and serialise only for the device part
-static void encrypt_asymmetric(Encryptor_ *e, const Plaintext_ &plain, b200::Blake2xbPrng &prng, Ciphertext_ &dst,
-                               std::unique_lock<std::mutex> &lk, bool disable_special_modulus = false, EncComponents *comp = nullptr)
-{
-    Context_ *c = e->ctx;
-    if (!e->has_pk)
-        throw LogicErr("public key is not set");
-    const size_t n = c->parms.n, K = c->parms.coeff.size();
-    const bool drop = c->first_level == 1 && !disable_special_modulus; // encrypt at the key level, then switch down
-    const int enc_lv = drop ? 0 : c->first_level;
-    const size_t ke = (size_t)c->level_k[enc_lv];
-    const std::vector<u64> mods(c->parms.coeff.begin(), c->parms.coeff.begin() + ke);
-    // u, e_0, e_1 as small signed values; their residues are formed on the device
-    std::vector<u64> us(n), es(2 * n);
-    WipeGuard wgu(us), wge(es);
-    b200::sample_poly_ternary(prng, n, signed_only(), us.data());
-    b200::sample_poly_normal(prng, n, signed_only(), es.data());
-    b200::sample_poly_normal(prng, n, signed_only(), es.data() + n);
-    lk.lock();
-    std::vector<u64> pv = padded_plain(c, plain);
-    if (comp)
-    {
-        if (comp->u)
-        {
-            comp->u->reserve(1, n, mods);
-            comp->u->insert(0, expand_signed_host(us.data(), n, mods).data());
-        }
-        if (comp->e)
-        {
-            comp->e->reserve(2, n, mods);
-            comp->e->insert(0, expand_signed_host(es.data(), n, mods).data());
-            comp->e->insert(1, expand_signed_host(es.data() + n, n, mods).data());
-        }
-    }
-    const u64 *dpk = e->dev_pk(enc_lv); // first ke residues of both public-key polynomials, resident
-    DevBuf dus(c, us), des(c, es), du(c, ke * n), de(c, 2 * ke * n), dct(c, 2 * ke * n), dpl(c, pv);
-    dev_check(b200_expand_signed(c->dev, enc_lv, (const int64_t *)dus.p, 1, du.p, nullptr));
-    dev_check(b200_expand_signed(c->dev, enc_lv, (const int64_t *)des.p, 2, de.p, nullptr));
-    dev_check(b200_ntt_forward(c->dev, enc_lv, du.p, 1, nullptr));
-    dev_check(b200_dyadic_product(c->dev, enc_lv, dpk, 2, du.p, 1, dct.p, 1, nullptr)); // pk_j (*) NTT(u)
-    dev_check(b200_ntt_inverse(c->dev, enc_lv, dct.p, 2, nullptr));                       // two polys = two slab items
-    dev_check(b200_add(c->dev, enc_lv, dct.p, de.p, dct.p, 2, 1, nullptr));               // + e_j
-    const int lv = c->first_level;
-    u64 *out = dst.prepare_output(c, c->ids[lv], 2, c->level_k[lv]);
-    if (drop)
-    {
-        DevBuf tmp(c, 2 * (K - 1) * n);
-        dev_check(b200_mod_switch_to_next(c->dev, 0, dct.p, 2, tmp.p, 1, nullptr));
-        dev_check(b200_add_plain(c->dev, lv, tmp.p, 2, dpl.p, 1, out, 1, nullptr));
-    }
-    else
-        dev_check(b200_add_plain(c->dev, lv, dct.p, 2, dpl.p, 1, out, 1, nullptr));
-    dev_check(b200_stream_synchronize(c->dev, nullptr));
-    if (comp && comp->remainder)
-        export_remainder(c, plain, *comp->remainder);
-}
-
-// sk encryption: encrypt_zero_symmetric at the first data level, coefficient form (S/util/rlwe.cpp:312-459), then
-// add round(q m / t).  `bootstrap` supplies the public seed of the uniform polynomial and the noise.
-static void encrypt_symmetric(Encryptor_ *e, const Plaintext_ &plain, b200::Blake2xbPrng &bootstrap, Ciphertext_ &dst,
-                              std::unique_lock<std::mutex> &lk, EncComponents *comp = nullptr)
-{
-    Context_ *c = e->ctx;
-    if (!e->has_sk)
-        throw LogicErr("secret key is not set");
-    const int lv = c->first_level;
-    const size_t n = c->parms.n;
-    const int k = c->level_k[lv];
-    std::vector<u64> mods(c->parms.coeff.begin(), c->parms.coeff.begin() + k);
-    b200::PrngSeed pub;
-    bootstrap.generate(sizeof(pub), pub.data());
-    b200::Blake2xbPrng ct_prng(pub);
-    std::vector<u64> c1((size_t)k * n), noise(n);
-    WipeGuard wgn(noise);
-    b200::sample_poly_uniform(ct_prng, n, mods, c1.data());
-    b200::sample_poly_normal(bootstrap, n, signed_only(), noise.data());
-    lk.lock();
-    std::vector<u64> pv = padded_plain(c, plain);
-    if (comp && comp->e)
-    {
-        comp->e->reserve(1, n, mods);
-        comp->e->insert(0, expand_signed_host(noise.data(), n, mods).data());
-    }
-    const u64 *dsk = e->dev_sk(); // [K][n] resident; the first k residues are this level's
-    DevBuf d1(c, c1), dn(c, noise), de(c, (size_t)k * n), d0(c, (size_t)2 * k * n), dpl(c, pv);
-    dev_check(b200_expand_signed(c->dev, lv, (const int64_t *)dn.p, 1, de.p, nullptr));
-    // c0 = -(INTT(s (*) c1) + e); c1 is sampled in the NTT domain and converted back at the end
-    dev_check(b200_dyadic_product(c->dev, lv, dsk, 1, d1.p, 1, d0.p, 1, nullptr));
-    dev_check(b200_ntt_inverse(c->dev, lv, d0.p, 1, nullptr));
-    dev_check(b200_add(c->dev, lv, d0.p, de.p, d0.p, 1, 1, nullptr));
-    dev_check(b200_negate(c->dev, lv, d0.p, d0.p, 1, 1, nullptr));
-    dev_check(b200_ntt_inverse(c->dev, lv, d1.p, 1, nullptr));
-    dev_check(b200_memcpy_d2d(c->dev, d0.p + (size_t)k * n, d1.p, (size_t)k * n * 8, nullptr));
-    u64 *out = dst.prepare_output(c, c->ids[lv], 2, k);
-    dev_check(b200_add_plain(c->dev, lv, d0.p, 2, dpl.p, 1, out, 1, nullptr));
-    dev_check(b200_stream_synchronize(c->dev, nullptr));
-    if (comp && comp->remainder)
-        export_remainder(c, plain, *comp->remainder);
-}
-
 // Encryptor_Encrypt{,Symmetric}ReturnComponents{,SetSeed} (S/c/encryptor.cpp:136-240,300-372): the fork's entry points
-// that also hand back u, e and the rounding remainder; `seed8` == nullptr draws a fresh seed
+// that also hand back u, e and the rounding remainder; `seed8` == nullptr draws a fresh seed.  u and e are the residues, at
+// the level the zero encryption is made at, of the samples layer 1 hands back.
 static long encrypt_components(void *p, void *plaintext, bool asymmetric, bool disable_special_modulus, void *destination,
                                void *u_dst, void *e_dst, void *r_dst, const uint64_t *seed8)
 {
     auto *e = (Encryptor_ *)p;
     return guard([&] {
-        std::unique_lock<std::mutex> lk(e->ctx->mu, std::defer_lock);
-        b200::PrngSeed sd = seed8 ? b200::PrngSeed{} : b200::random_seed();
-        if (seed8)
-            std::copy_n(seed8, 8, sd.begin());
-        b200::Blake2xbPrng prng(sd);
+        Context_ *c = e->ctx;
         EncComponents comp{ (PolynomialArray_ *)u_dst, (PolynomialArray_ *)e_dst, (Plaintext_ *)r_dst };
         // the component arrays must be fresh: reserve() refuses a second use, like the reference's
         if ((comp.u && comp.u->reserved) || (comp.e && comp.e->reserved))
             throw LogicErr("PolynomialArray can only be reserved once.");
-        if (asymmetric)
-            encrypt_asymmetric(e, *(Plaintext_ *)plaintext, prng, *(Ciphertext_ *)destination, lk, disable_special_modulus, &comp);
-        else
-            encrypt_symmetric(e, *(Plaintext_ *)plaintext, prng, *(Ciphertext_ *)destination, lk, &comp);
+        const size_t n = c->parms.n;
+        EncSamples S;
+        encrypt_batch(e, 1, &plaintext, seed8, !asymmetric, disable_special_modulus, &destination, S);
+        const int8_t *smp = S.small.data();
+        // pk: encrypted at the key level unless the special modulus is disabled (S/encryptor.cpp:160-163)
+        const int enc_lv = asymmetric && c->first_level == 1 && !disable_special_modulus ? 0 : c->first_level;
+        const std::vector<u64> mods(c->parms.coeff.begin(), c->parms.coeff.begin() + c->level_k[enc_lv]);
+        if (comp.u)
+        {
+            comp.u->reserve(1, n, mods);
+            comp.u->insert(0, expand_signed_host(smp, n, mods).data());
+        }
+        if (comp.e)
+        {
+            const size_t polys = asymmetric ? 2 : 1, first = asymmetric ? 1 : 0;
+            comp.e->reserve(polys, n, mods);
+            for (size_t j = 0; j < polys; j++)
+                comp.e->insert(j, expand_signed_host(smp + (first + j) * n, n, mods).data());
+        }
+        if (comp.remainder)
+            export_remainder(c, *(Plaintext_ *)plaintext, *comp.remainder);
     });
 }
 long Encryptor_EncryptReturnComponents(void *p, void *plaintext, bool disable_special_modulus, void *destination, void *u_dst,
@@ -3359,11 +3377,9 @@ long Encryptor_Encrypt(void *p, void *plaintext, void *destination, void *)
     NULLRET(p);
     NULLRET(plaintext);
     NULLRET(destination);
-    auto *e = (Encryptor_ *)p;
     return guard([&] {
-        std::unique_lock<std::mutex> lk(e->ctx->mu, std::defer_lock);
-        b200::Blake2xbPrng prng(b200::random_seed());
-        encrypt_asymmetric(e, *(Plaintext_ *)plaintext, prng, *(Ciphertext_ *)destination, lk);
+        EncSamples S;
+        encrypt_batch((Encryptor_ *)p, 1, &plaintext, nullptr, false, false, &destination, S);
     });
 }
 // deterministic variant: same stream as the reference's Encryptor_EncryptReturnComponentsSetSeed (S/c/encryptor.cpp:185-240)
@@ -3373,13 +3389,9 @@ long B200_Encryptor_EncryptSetSeed(void *p, void *plaintext, const uint64_t *see
     NULLRET(plaintext);
     NULLRET(seed8);
     NULLRET(destination);
-    auto *e = (Encryptor_ *)p;
     return guard([&] {
-        std::unique_lock<std::mutex> lk(e->ctx->mu, std::defer_lock);
-        b200::PrngSeed sd;
-        std::copy_n(seed8, 8, sd.begin());
-        b200::Blake2xbPrng prng(sd);
-        encrypt_asymmetric(e, *(Plaintext_ *)plaintext, prng, *(Ciphertext_ *)destination, lk);
+        EncSamples S;
+        encrypt_batch((Encryptor_ *)p, 1, &plaintext, seed8, false, false, &destination, S);
     });
 }
 long Encryptor_EncryptSymmetric(void *p, void *plaintext, bool /*save_seed*/, void *destination, void *)
@@ -3389,11 +3401,57 @@ long Encryptor_EncryptSymmetric(void *p, void *plaintext, bool /*save_seed*/, vo
     NULLRET(p);
     NULLRET(plaintext);
     NULLRET(destination);
-    auto *e = (Encryptor_ *)p;
     return guard([&] {
-        std::unique_lock<std::mutex> lk(e->ctx->mu, std::defer_lock);
-        b200::Blake2xbPrng bootstrap(b200::random_seed());
-        encrypt_symmetric(e, *(Plaintext_ *)plaintext, bootstrap, *(Ciphertext_ *)destination, lk);
+        EncSamples S;
+        encrypt_batch((Encryptor_ *)p, 1, &plaintext, nullptr, true, false, &destination, S);
+    });
+}
+long B200_Encryptor_EncryptBatch(void *encryptor, uint64_t count, void **plains, const uint64_t *seeds, bool symmetric,
+                                 void **destinations)
+{
+    NULLRET(encryptor);
+    NULLRET(plains);
+    NULLRET(destinations);
+    return guard([&] {
+        batch_handles(count, { plains, destinations });
+        distinct_destinations(count, destinations);
+        EncSamples S;
+        encrypt_batch((Encryptor_ *)encryptor, count, plains, seeds, symmetric, false, destinations, S);
+    });
+}
+long B200_Encryptor_EncryptSlotsBatch(void *encryptor, void *encoder, uint64_t count, uint64_t values_per_item,
+                                      const uint64_t *values, bool is_signed, const uint64_t *seeds, bool symmetric,
+                                      void **destinations)
+{
+    NULLRET(encryptor);
+    NULLRET(encoder);
+    NULLRET(destinations);
+    if (count && values_per_item)
+        NULLRET(values);
+    auto *e = (Encryptor_ *)encryptor;
+    Context_ *c = e->ctx;
+    if (((BatchEncoder_ *)encoder)->ctx != c)
+        return E_INVALIDARG_;
+    return guard([&] {
+        batch_handles(count, { destinations });
+        distinct_destinations(count, destinations);
+        if (!c->using_batching)
+            throw InvalidArg("encryption parameters are not valid for batching");
+        encrypt_key_check(e, symmetric);
+        if (values_per_item > c->parms.n)
+            throw InvalidArg("values_matrix size is too large");
+        if (count == 0)
+            return;
+        EncSamples S;
+        encrypt_sample(c, count, seeds, symmetric, S);
+        SeamScope scope(c);
+        const size_t n = c->parms.n;
+        BatchSlab V(c, count * values_per_item), P(c, count * n);
+        if (values_per_item)
+            dev_check(b200_memcpy_h2d(c->dev, V.p, values, count * values_per_item * sizeof(u64), cur_stream()));
+        dev_check(b200_batch_encode(c->dev, V.w(), values_per_item, is_signed ? 1 : 0, P.w(), count, cur_stream()));
+        encrypt_device(e, count, P, S, symmetric, false, destinations);
+        scope.wait();
     });
 }
 

@@ -701,13 +701,13 @@ inline const std::vector<u64> &signed_only()
     static const std::vector<u64> z(1, 0);
     return z;
 }
-// host-side residues of such signed samples (only where the caller wants the components back: PolynomialArray)
-inline std::vector<u64> expand_signed_host(const u64 *vals, size_t n, const std::vector<u64> &mods)
+// host-side residues of small signed samples (only where the caller wants the components back: PolynomialArray)
+inline std::vector<u64> expand_signed_host(const int8_t *vals, size_t n, const std::vector<u64> &mods)
 {
     std::vector<u64> out(mods.size() * n);
     for (size_t i = 0; i < mods.size(); i++)
         for (size_t c = 0; c < n; c++)
-            out[i * n + c] = (int64_t)vals[c] < 0 ? vals[c] + mods[i] : vals[c];
+            out[i * n + c] = vals[c] < 0 ? mods[i] - (u64)(-vals[c]) : (u64)vals[c];
     return out;
 }
 
@@ -790,21 +790,16 @@ struct Encryptor_
     std::vector<u64> pk; // [2][K][n] NTT form, key level
     std::vector<u64> sk; // [K][n]
     ~Encryptor_() { wipe(sk); }
-    DevCache dev_cache;  // key 0: secret key [K][n]; key 1 + level: the level's residues of both public-key polynomials
+    DevCache dev_cache;  // key 0: secret key [K][n]; key 1: public key [2][K][n]
     const u64 *dev_sk()
     {
         u64 *p = dev_cache.find(0);
         return p ? p : dev_cache.put(ctx, 0, sk);
     }
-    const u64 *dev_pk(int level)
+    const u64 *dev_pk()
     {
-        if (u64 *p = dev_cache.find(1 + level))
-            return p;
-        const size_t n = ctx->parms.n, K = ctx->parms.coeff.size(), ke = (size_t)ctx->level_k[level];
-        std::vector<u64> part(2 * ke * n);
-        for (int j = 0; j < 2; j++)
-            std::copy_n(pk.begin() + (size_t)j * K * n, ke * n, part.begin() + (size_t)j * ke * n);
-        return dev_cache.put(ctx, 1 + level, part);
+        u64 *p = dev_cache.find(1);
+        return p ? p : dev_cache.put(ctx, 1, pk);
     }
 };
 

@@ -89,6 +89,12 @@ _SIGS = {
     "b200_batch_encode": [vp, vp, u64, C.c_int, vp, u64, vp],
     "b200_batch_decode": [vp, vp, C.c_int, vp, u64, vp],
     "b200_decrypt_slots": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, u64, vp],
+    "b200_sample_pk": [vp, vp, vp, u64],
+    "b200_sample_sk": [vp, vp, vp, vp, u64],
+    "b200_encrypt_pk_samples": [vp, vp, vp, vp, C.c_int, vp, u64, vp],
+    "b200_encrypt_sk_samples": [vp, vp, vp, vp, vp, vp, u64, vp],
+    "b200_encrypt_pk": [vp, vp, vp, vp, C.c_int, vp, vp, u64, vp],
+    "b200_encrypt_sk": [vp, vp, vp, vp, vp, vp, u64, vp],
     "b200_is_transparent": [vp, C.c_int, vp, C.c_int, vp, u64, vp],
     "b200_any_nonzero": [vp, C.c_int, vp, C.c_int, vp, u64, vp],
     "b200_expand_signed": [vp, C.c_int, vp, C.c_int, vp, vp],
@@ -356,6 +362,37 @@ class B200Context:
         one secret-key phase (the call then returns after completion)."""
         self.L.call("b200_decrypt_slots", self.h, self._lv(level), vp(ptr(ct)), C.c_int(size), vp(ptr(sk_powers)),
                     C.c_int(1 if signed else 0), vp(ptr(slots_out)), vp(ptr(norm_out_host)), C.c_int(words), u64(batch), vp(stream))
+
+    def sample_pk(self, seeds, samples_out, batch):
+        """host step of encrypt_pk: u, e0, e1 of each item into samples_out (HOST int8 [batch][3][n])."""
+        self.L.call("b200_sample_pk", self.h, vp(ptr(seeds)), vp(ptr(samples_out)), u64(batch))
+
+    def sample_sk(self, seeds, c1_out, noise_out, batch):
+        """host step of encrypt_sk: c1 (HOST uint64 [batch][k1][n], NTT form) and e (HOST int8 [batch][n])."""
+        self.L.call("b200_sample_sk", self.h, vp(ptr(seeds)), vp(ptr(c1_out)), vp(ptr(noise_out)), u64(batch))
+
+    def encrypt_pk_samples(self, pk, samples, plain, out, batch, disable_special_modulus=False, stream=None):
+        """device step of encrypt_pk from sample_pk's samples (asynchronous: keep `samples` until the stream has passed)."""
+        self.L.call("b200_encrypt_pk_samples", self.h, vp(ptr(pk)), vp(ptr(samples)), vp(ptr(plain)),
+                    C.c_int(1 if disable_special_modulus else 0), vp(ptr(out)), u64(batch), vp(stream))
+
+    def encrypt_sk_samples(self, sk, c1, noise, plain, out, batch, stream=None):
+        """device step of encrypt_sk from sample_sk's c1 and e (asynchronous, as encrypt_pk_samples)."""
+        self.L.call("b200_encrypt_sk_samples", self.h, vp(ptr(sk)), vp(ptr(c1)), vp(ptr(noise)), vp(ptr(plain)), vp(ptr(out)),
+                    u64(batch), vp(stream))
+
+    def encrypt_pk(self, pk, seeds, plain, out, batch, disable_special_modulus=False, samples_out=None, stream=None):
+        """pk [2][K][n] NTT form at the key level, plain [batch][n] mod t -> out [batch][2][k1][n] at the first data level;
+        item i draws u, e0, e1 from the 8-word seeds[i] (HOST uint64 [batch][8]) as Encryptor_EncryptReturnComponentsSetSeed.
+        samples_out: None or HOST int8 [batch][3][n] receiving u, e0, e1.  Returns after completion."""
+        self.L.call("b200_encrypt_pk", self.h, vp(ptr(pk)), vp(ptr(seeds)), vp(ptr(plain)), C.c_int(1 if disable_special_modulus else 0),
+                    vp(ptr(out)), vp(ptr(samples_out)), u64(batch), vp(stream))
+
+    def encrypt_sk(self, sk, seeds, plain, out, batch, noise_out=None, stream=None):
+        """sk [K][n] NTT form, plain [batch][n] mod t -> out [batch][2][k1][n], item i as
+        Encryptor_EncryptSymmetricReturnComponentsSetSeed with seeds[i]; noise_out: None or HOST int8 [batch][n] (e)."""
+        self.L.call("b200_encrypt_sk", self.h, vp(ptr(sk)), vp(ptr(seeds)), vp(ptr(plain)), vp(ptr(out)), vp(ptr(noise_out)),
+                    u64(batch), vp(stream))
 
     def is_transparent(self, ct, size, flags, batch, level=None, stream=None):
         self.L.call("b200_is_transparent", self.h, self._lv(level), vp(ptr(ct)), C.c_int(size), vp(ptr(flags)), u64(batch),
